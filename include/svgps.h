@@ -214,10 +214,11 @@ int sv_embedding_bwd(const void *grad_out, long long ldg, int is_bf16, const lon
 
 /* clip_grad_norm_ + AdamW + bf16 shadow refresh over FLAT buffers in two launches (squared-norm partials, then the update;
  * reference: trainer/build.py:135-145, optim/utils.py:1-18).  params / exp_avg / exp_avg_sq / grads: n f32, 16-byte aligned;
- * shadow_bf16: n bf16 (may be NULL).  segments: DEVICE array of nseg records {long long begin, end; float lr_scale,
- * weight_decay} (element ranges, multiples of 4) — lr of a segment = base_lr * lr_scale * *lr_factor.  step: device 1-based
- * step counter (bias correction).  scratch: sv_adamw_scratch_floats() floats.  norm_out (may be NULL) receives ||g||.
- * max_norm <= 0 disables clipping. */
+ * shadow_bf16: n bf16, 8-byte aligned (may be NULL).  segments: DEVICE array of nseg records {long long begin, end; float
+ * lr_scale, weight_decay} (element ranges, multiples of 4), 8-byte aligned — lr of a segment = base_lr * lr_scale * *lr_factor.
+ * step: device 1-based step counter (bias correction).  scratch: sv_adamw_scratch_floats() floats.  norm_out (may be NULL)
+ * receives ||g||.  max_norm <= 0 disables clipping.  A non-finite norm poisons the update as it does in clip_grad_norm_: NaN
+ * makes every updated element NaN, inf gives a clip factor of 0. */
 int sv_adamw_scratch_floats(void);
 int sv_adamw_flat(float *params, float *exp_avg, float *exp_avg_sq, const float *grads, void *shadow_bf16, long long n,
                   const void *segments, int nseg, float max_norm, const float *lr_factor, const long long *step, float base_lr,

@@ -153,7 +153,9 @@ __global__ void __launch_bounds__(256) adamw_flat_kernel(const AdamArgs a) {
     float tot = 0.f;
     for (int i = 0; i < a.npart; ++i) tot += a.partials[i];   // fixed order: deterministic
     const float nrm = sqrtf(tot);
-    s_clip = a.max_norm > 0.f ? fminf(1.0f, a.max_norm / (nrm + 1e-6f)) : 1.0f;
+    // not fminf: it would turn a NaN norm into 1 and apply an unclipped update; clamp(max=1) in clip_grad_norm_ keeps the NaN
+    const float c = a.max_norm / (nrm + 1e-6f);
+    s_clip = a.max_norm > 0.f ? (c > 1.0f ? 1.0f : c) : 1.0f;
     const double st = (double)*a.step;
     s_bc1 = (float)(1.0 - pow((double)a.beta1, st));
     s_bc2s = (float)sqrt(1.0 - pow((double)a.beta2, st));
@@ -239,8 +241,9 @@ extern "C" int sv_adamw_flat(float *params, float *exp_avg, float *exp_avg_sq, c
   if (n == 0 || nseg == 0) return SV_OK;
   if (!params || !exp_avg || !exp_avg_sq || !grads || !segments || !lr_factor || !step || !scratch) return SV_ERR_INVALID_ARG;
   if ((reinterpret_cast<uintptr_t>(params) & 15) || (reinterpret_cast<uintptr_t>(grads) & 15) ||
-      (reinterpret_cast<uintptr_t>(exp_avg) & 15) || (reinterpret_cast<uintptr_t>(exp_avg_sq) & 15))
-    return SV_ERR_INVALID_ARG;
+      (reinterpret_cast<uintptr_t>(exp_avg) & 15) || (reinterpret_cast<uintptr_t>(exp_avg_sq) & 15) ||
+      (reinterpret_cast<uintptr_t>(shadow_bf16) & 7) || (reinterpret_cast<uintptr_t>(segments) & 7))
+    return SV_ERR_INVALID_ARG;   // the shadow is written as uint2, the segment records are read as 8-byte fields
   cudaStream_t st = (cudaStream_t)stream;
   const int npart = 528;  // 132 SMs (H100 SXM) x 4
   sqnorm_partial_kernel<<<npart, 512, 0, st>>>(grads, n, scratch);

@@ -393,11 +393,10 @@ class _EmbeddingFn(torch.autograd.Function):
             total = native.colsum(g2 if g2.dtype in (torch.bfloat16, torch.float32) else g2.float())
             rest = torch.zeros_like(total)
             for v in range(1, weight.shape[0]):
-                if pad is not None and v == pad:
-                    continue
                 part = native.colsum((g2 * (flat == v).unsqueeze(1).to(g2.dtype)).contiguous())
-                dw[v] += part
-                rest += part
+                rest += part            # the padding row's tokens too: row 0 gets total - rest
+                if pad is None or v != pad:
+                    dw[v] += part
             if pad is None or pad != 0:
                 dw[0] += total - rest
         else:
