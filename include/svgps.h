@@ -243,6 +243,29 @@ int sv_pn_bn_relu_fwd(const void *y, long long R, int C, const float *gamma, con
                       float *var_unbiased, void *out, float *scratch, void *stream);
 int sv_pn_bn_relu_bwd(const void *y, const void *dout, long long R, int C, const float *gamma, const float *beta, const float *mean,
                       const float *rstd, void *dy, float *dgamma, float *dbeta, int accumulate, float *scratch, void *stream);
+/* The same layer with SyncBatchNorm statistics over `world` ranks (reference: model/objcls.py:33-34 convert_sync_batchnorm;
+ * torch.nn.SyncBatchNorm semantics: mean / variance over the rows of all ranks, d gamma / d beta stay this rank's sums, dY uses
+ * the global sums and 1 / R_total).  Each BatchNorm pass is two launches, push then finish, so that ranks exchange their column
+ * sums in between:
+ *   push (mode 0: sum y, sum y^2; mode 1: sum g', sum g' * xhat with the global mean / rstd) reduces this rank's R rows (R = 0
+ *   allowed) to fp64 and stores [sum0 (C) | sum1 (C) | R] into this rank's slot of every rank's exchange buffer, then raises
+ *   this rank's flag on every rank;
+ *   finish waits for every rank's flag, sums the slots in rank order (bit-identical on every rank) and applies the layer.
+ * peer_bufs: DEVICE array of `world` device pointers to the ranks' exchange buffers (8-byte aligned), each
+ * sv_pn_sync_floats(cap, world) floats, zero-initialised, with C <= cap; one buffer serves every layer on one stream.
+ * epoch_dev: zero-initialised device word of this rank: push uses *epoch_dev + 1, finish stores it back (CUDA-graph replay).
+ * done_counter: zero-initialised device word, reset by push.  scratch: sv_pn_scratch_floats(C).  gsum: (2C + 1) f32 out, the
+ * global sums and 1 / R_total that the dY kernel reads.  Returns 0 floats for an invalid C or world. */
+int sv_pn_sync_floats(int C, int world);
+int sv_pn_bn_sync_push(int mode, const void *y, const void *dout, long long R, int C, const float *gamma, const float *beta,
+                       const float *mean, const float *rstd, float *scratch, void *const *peer_bufs, int cap, unsigned *done_counter,
+                       int world, int rank, const unsigned *epoch_dev, void *stream);
+int sv_pn_bn_sync_finish_fwd(const void *y, long long R, int C, const float *gamma, const float *beta, float eps, float *mean,
+                             float *rstd, float *var_unbiased, void *out, void *const *peer_bufs, int cap, int world, int rank,
+                             unsigned *epoch_dev, void *stream);
+int sv_pn_bn_sync_finish_bwd(const void *y, const void *dout, long long R, int C, const float *gamma, const float *beta,
+                             const float *mean, const float *rstd, void *dy, float *dgamma, float *dbeta, int accumulate, float *gsum,
+                             void *const *peer_bufs, int cap, int world, int rank, unsigned *epoch_dev, void *stream);
 /* out[g][c] = max over the ns rows of group g, arg = index of the first maximum (bytes, ns <= 255); grad: gx[g*ns+s][c] = gout[g][c]
  * where s == arg, else 0. */
 int sv_pn_rowgroup_max(const void *x, long long G, int ns, int C, void *out, unsigned char *arg, void *stream);

@@ -131,6 +131,13 @@ _GPS_SIGS = {
                           c_void_p, c_void_p],
     "sv_pn_bn_relu_bwd": [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                           c_void_p, c_int, c_void_p, c_void_p],
+    "sv_pn_sync_floats": [c_int, c_int],
+    "sv_pn_bn_sync_push": [c_int, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                           c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p],
+    "sv_pn_bn_sync_finish_fwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p,
+                                 c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
+    "sv_pn_bn_sync_finish_bwd": [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
     "sv_pn_rowgroup_max": [c_void_p, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "sv_pn_rowgroup_max_grad": [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p],
     "sv_sa_mlp_param_bytes": [c_int],

@@ -222,8 +222,9 @@ def warmup_cosine(step, warmup_step, total_step, minimum_ratio=1e-5):
 class ObjCls(nn.Module):
     """Object-level pre-training model (reference: model/objcls.py:16-98), `model_name='pointnet++'`, open-vocabulary
     head against the 607 frozen text embeddings, bert language type (768-d).  PointNet++ is trainable here with
-    train-mode BatchNorm (SyncBatchNorm when num_gpu > 1, objcls.py:33-34), so it runs the generic operator sequence on
-    the native point ops — the one shipped path that needs `group_points_grad` (SURVEY.md §3.4)."""
+    train-mode BatchNorm (SyncBatchNorm when num_gpu > 1, objcls.py:33-34) on the channels-last native path of pn_train.py;
+    SyncBatchNorm exchanges its statistics through pn_train.StatExchange (the generic operator sequence on the native point
+    ops remains the fallback)."""
 
     def __init__(self, cfg, text_embeds=None):
         super().__init__()

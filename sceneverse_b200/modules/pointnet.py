@@ -151,7 +151,7 @@ class PointNetPP(nn.Module):
 
     # -------------------------------------------------------------- helpers
     def _bn_all_eval(self):
-        return all(not m.training for m in self.modules() if isinstance(m, nn.BatchNorm2d))
+        return all(not m.training for m in self.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm))
 
     def fused_available(self, pts):
         return (self.spec == GPS_SPEC and pts.is_cuda and pts.dtype == torch.float32 and pts.size(-1) == 6

@@ -56,28 +56,137 @@ class _GroupRowsFn(torch.autograd.Function):
         return None, None, dfeat.to(fdt), None, None, None
 
 
+class StatExchange:
+    """The column-sum exchange of the SyncBatchNorm layers (csrc/pn_train.cu sv_pn_bn_sync_*; reference: model/objcls.py:33-34
+    convert_sync_batchnorm): one symmetric buffer per (device, process group) on top of torch's symmetric-memory allocator, sized
+    for C <= CAP and shared by every BatchNorm layer of the backbone — the layers run one after another on one stream, and the
+    kernels double-buffer by the parity of the device-resident epoch (each push / finish pair is one exchange)."""
+    CAP = 768
+
+    def __init__(self, device, group=None, local=False):
+        """local=True: world 1 on an ordinary device buffer, no process group — the same kernels, flags and parity logic."""
+        lib = _lib.gps()
+        if local:
+            self.group, world, rank = None, 1, 0
+            self.buf = torch.zeros(lib.sv_pn_sync_floats(self.CAP, 1), dtype=torch.float32, device=device)
+            ptrs = [self.buf.data_ptr()]
+        else:
+            import torch.distributed as dist
+            import torch.distributed._symmetric_memory as symm_mem
+            self.group = group or dist.group.WORLD
+            world, rank = dist.get_world_size(self.group), dist.get_rank(self.group)
+            self.buf = symm_mem.empty(lib.sv_pn_sync_floats(self.CAP, world), dtype=torch.float32, device=device)
+            self.buf.zero_()
+            self.hdl = symm_mem.rendezvous(self.buf, self.group.group_name)
+            ptrs = [int(p) for p in self.hdl.buffer_ptrs]
+        self._setup(ptrs, world, rank, device)
+        torch.cuda.synchronize(device)
+        if not local:
+            import torch.distributed as dist
+            dist.barrier(self.group)      # every rank's buffer (flags included) is zeroed before the first push
+
+    def _setup(self, ptrs, world, rank, device):
+        self.world, self.rank = world, rank
+        self.peer_bufs = torch.tensor(ptrs, dtype=torch.int64, device=device)
+        self.done = torch.zeros(1, dtype=torch.int32, device=device)
+        self.epoch_dev = torch.zeros(1, dtype=torch.int32, device=device)   # exchanges completed by this rank (graph-replay safe)
+
+    @classmethod
+    def emulated(cls, k, device):
+        """Tests only: k ranks on ONE device, each with its own buffer, epoch and done counter, sharing one peer table.  Run
+        every rank's push before any rank's finish (one stream): then every flag is already set and no kernel waits."""
+        lib = _lib.gps()
+        bufs = [torch.zeros(lib.sv_pn_sync_floats(cls.CAP, k), dtype=torch.float32, device=device) for _ in range(k)]
+        out = []
+        for r in range(k):
+            ex = cls.__new__(cls)
+            ex.group, ex.buf, ex._all = None, bufs[r], bufs
+            ex._setup([b.data_ptr() for b in bufs], k, r, device)
+            out.append(ex)
+        return out
+
+    def push(self, mode, y, dout=None, stats=None, g32=None, b32=None):
+        """mode 0: this rank's column sums of y; mode 1: of g' and g' * xhat (stats = the global mean, rstd)."""
+        R, C = y.shape
+        assert C <= self.CAP
+        lib = _lib.gps()
+        scratch = torch.empty(lib.sv_pn_scratch_floats(C), dtype=torch.float32, device=y.device)
+        p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        with torch.cuda.device(y.device):
+            st = lib.sv_pn_bn_sync_push(mode, p(y), p(dout), R, C, p(g32), p(b32), p(stats[0]) if stats is not None else None,
+                                        p(stats[1]) if stats is not None else None, scratch.data_ptr(), self.peer_bufs.data_ptr(),
+                                        self.CAP, self.done.data_ptr(), self.world, self.rank, self.epoch_dev.data_ptr(), _st(y))
+        _lib.check(lib, st, "sv_pn_bn_sync_push")
+
+    def finish_fwd(self, y, g32, b32, eps):
+        """-> (relu(BN(y)) bf16, stats (3, C) f32: global mean, rstd, unbiased variance)."""
+        R, C = y.shape
+        stats = torch.empty((3, C), dtype=torch.float32, device=y.device)
+        out = torch.empty_like(y)
+        lib = _lib.gps()
+        with torch.cuda.device(y.device):
+            st = lib.sv_pn_bn_sync_finish_fwd(y.data_ptr(), R, C, g32.data_ptr(), b32.data_ptr(), float(eps), stats[0].data_ptr(),
+                                              stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(), self.peer_bufs.data_ptr(),
+                                              self.CAP, self.world, self.rank, self.epoch_dev.data_ptr(), _st(y))
+        _lib.check(lib, st, "sv_pn_bn_sync_finish_fwd")
+        return out, stats
+
+    def finish_bwd(self, y, dout, stats, g32, b32):
+        """-> (dy bf16, dgb (2, C) f32: this rank's d gamma, d beta)."""
+        R, C = y.shape
+        dy = torch.empty_like(y)
+        dgb = torch.empty((2, C), dtype=torch.float32, device=y.device)
+        gsum = torch.empty(2 * C + 1, dtype=torch.float32, device=y.device)
+        lib = _lib.gps()
+        with torch.cuda.device(y.device):
+            st = lib.sv_pn_bn_sync_finish_bwd(y.data_ptr(), dout.data_ptr(), R, C, g32.data_ptr(), b32.data_ptr(), stats[0].data_ptr(),
+                                              stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(), 0,
+                                              gsum.data_ptr(), self.peer_bufs.data_ptr(), self.CAP, self.world, self.rank,
+                                              self.epoch_dev.data_ptr(), _st(y))
+        _lib.check(lib, st, "sv_pn_bn_sync_finish_bwd")
+        return dy, dgb
+
+
 class _ConvBNReLUFn(torch.autograd.Function):
-    """out = relu(BatchNorm_batchstats(X W^T)): X (R,Kp) bf16 (zero-padded columns), W = conv.weight (Cout,Cin,1,1) f32."""
+    """out = relu(BatchNorm_batchstats(X W^T)): X (R,Kp) bf16 (zero-padded columns), W = conv.weight (Cout,Cin,1,1) f32.
+    ex: a StatExchange for SyncBatchNorm statistics over its ranks (push, then finish, in each direction), or None."""
 
     @staticmethod
-    def forward(ctx, X, weight, gamma, beta, eps):
+    def conv_fwd(X, weight):
         Cout, Cin = weight.shape[0], weight.shape[1]
-        R, Kp = X.shape
+        Kp = X.shape[1]
         wb = weight.detach().reshape(Cout, Cin).to(torch.bfloat16)
         if Kp != Cin:
             wb = F.pad(wb, (0, Kp - Cin))
-        y = native.linear_fwd(X, wb.contiguous())
+        wb = wb.contiguous()
+        return wb, native.linear_fwd(X, wb)
+
+    @staticmethod
+    def conv_bwd(X, wb, dy, cin, need_dx=True):
+        dX = native.linear_dgrad(dy, wb) if need_dx else None
+        dw, _ = native.linear_wgrad(dy, X)
+        return dX, dw[:, :cin].reshape(dy.shape[1], cin, 1, 1)
+
+    @staticmethod
+    def forward(ctx, X, weight, gamma, beta, eps, ex=None):
+        Cout, Cin = weight.shape[0], weight.shape[1]
+        R = X.shape[0]
+        wb, y = _ConvBNReLUFn.conv_fwd(X, weight)
         g32, b32 = gamma.detach().float().contiguous(), beta.detach().float().contiguous()
-        stats = torch.empty((3, Cout), dtype=torch.float32, device=X.device)     # mean, rstd, unbiased variance
-        out = torch.empty_like(y)
-        lib = _lib.gps()
-        scratch = torch.empty(lib.sv_pn_scratch_floats(Cout), dtype=torch.float32, device=X.device)
-        with torch.cuda.device(X.device):
-            st = lib.sv_pn_bn_relu_fwd(y.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), float(eps), stats[0].data_ptr(),
-                                       stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(), scratch.data_ptr(), _st(X))
-        _lib.check(lib, st, "sv_pn_bn_relu_fwd")
+        if ex is not None:
+            ex.push(0, y)
+            out, stats = ex.finish_fwd(y, g32, b32, eps)
+        else:
+            stats = torch.empty((3, Cout), dtype=torch.float32, device=X.device)     # mean, rstd, unbiased variance
+            out = torch.empty_like(y)
+            lib = _lib.gps()
+            scratch = torch.empty(lib.sv_pn_scratch_floats(Cout), dtype=torch.float32, device=X.device)
+            with torch.cuda.device(X.device):
+                st = lib.sv_pn_bn_relu_fwd(y.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), float(eps), stats[0].data_ptr(),
+                                           stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(), scratch.data_ptr(), _st(X))
+            _lib.check(lib, st, "sv_pn_bn_relu_fwd")
         ctx.save_for_backward(X, wb, y, stats, g32, b32)
-        ctx.cin = Cin
+        ctx.cin, ctx.ex = Cin, ex
         ctx.mark_non_differentiable(stats)
         return out, stats
 
@@ -86,19 +195,21 @@ class _ConvBNReLUFn(torch.autograd.Function):
         X, wb, y, stats, g32, b32 = ctx.saved_tensors
         R, Cout = y.shape
         dout = dout.contiguous()
-        dy = torch.empty_like(y)
-        dgb = torch.empty((2, Cout), dtype=torch.float32, device=y.device)
-        lib = _lib.gps()
-        scratch = torch.empty(lib.sv_pn_scratch_floats(Cout), dtype=torch.float32, device=y.device)
-        with torch.cuda.device(y.device):
-            st = lib.sv_pn_bn_relu_bwd(y.data_ptr(), dout.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), stats[0].data_ptr(),
-                                       stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(), 0,
-                                       scratch.data_ptr(), _st(y))
-        _lib.check(lib, st, "sv_pn_bn_relu_bwd")
-        dX = native.linear_dgrad(dy, wb) if ctx.needs_input_grad[0] else None
-        dw, _ = native.linear_wgrad(dy, X)
-        dw = dw[:, :ctx.cin].reshape(Cout, ctx.cin, 1, 1)
-        return dX, dw, dgb[0], dgb[1], None
+        if ctx.ex is not None:
+            ctx.ex.push(1, y, dout, stats, g32, b32)
+            dy, dgb = ctx.ex.finish_bwd(y, dout, stats, g32, b32)
+        else:
+            dy = torch.empty_like(y)
+            dgb = torch.empty((2, Cout), dtype=torch.float32, device=y.device)
+            lib = _lib.gps()
+            scratch = torch.empty(lib.sv_pn_scratch_floats(Cout), dtype=torch.float32, device=y.device)
+            with torch.cuda.device(y.device):
+                st = lib.sv_pn_bn_relu_bwd(y.data_ptr(), dout.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), stats[0].data_ptr(),
+                                           stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(), 0,
+                                           scratch.data_ptr(), _st(y))
+            _lib.check(lib, st, "sv_pn_bn_relu_bwd")
+        dX, dw = _ConvBNReLUFn.conv_bwd(X, wb, dy, ctx.cin, ctx.needs_input_grad[0])
+        return dX, dw, dgb[0], dgb[1], None, None
 
 
 class _RowGroupMaxFn(torch.autograd.Function):
@@ -139,17 +250,52 @@ def _update_running_stats(bn, stats):
             bn.running_var.mul_(1 - m).add_(stats[2].to(bn.running_var.dtype), alpha=m)
 
 
+_exchanges = {}
+
+
+def exchange_for(net, device):
+    """The StatExchange the net's train-mode BatchNorm layers need on `device`: None when their statistics are local (plain
+    BatchNorm2d, or SyncBatchNorm without an initialised process group or over one rank — torch's SyncBatchNorm normalises with
+    local statistics then too); False when the layers name different process groups or symmetric memory cannot be set up."""
+    syncs = [m for m in net.modules() if isinstance(m, torch.nn.SyncBatchNorm)]
+    if not syncs:
+        return None
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    groups = {id(m.process_group or dist.group.WORLD): m.process_group or dist.group.WORLD for m in syncs}
+    if len(groups) != 1:
+        return False
+    (group,) = groups.values()
+    if dist.get_world_size(group) == 1:
+        return None
+    key = (str(torch.device(device)), group.group_name)
+    if key not in _exchanges:
+        try:
+            _exchanges[key] = StatExchange(device, group)
+        except Exception as e:  # no P2P / unsupported allocator: the generic path with torch's SyncBatchNorm is used instead
+            _exchanges[key] = False
+            if dist.get_rank() == 0:
+                print(f"[sceneverse_b200] native SyncBatchNorm exchange unavailable ({type(e).__name__}: {e}); "
+                      "using the generic PointNet++ path")
+    return _exchanges[key]
+
+
 def available(pc, net):
-    """Train-mode BatchNorm (or a backbone that needs gradients) on CUDA under bf16 autocast."""
+    """Train-mode BatchNorm (or a backbone that needs gradients) on CUDA under bf16 autocast; SyncBatchNorm layers need their
+    exchange (exchange_for)."""
     if not (pc.is_cuda and pc.dtype == torch.float32 and torch.is_autocast_enabled("cuda")
             and torch.get_autocast_dtype("cuda") == torch.bfloat16):
         return False
-    bns = [m for m in net.modules() if isinstance(m, torch.nn.BatchNorm2d)]
-    return all(type(m) is torch.nn.BatchNorm2d and m.training and m.affine for m in bns)
+    bns = [m for m in net.modules() if isinstance(m, torch.nn.modules.batchnorm._BatchNorm)]
+    if not all(type(m) in (torch.nn.BatchNorm2d, torch.nn.SyncBatchNorm) and m.training and m.affine for m in bns):
+        return False
+    return exchange_for(net, pc.device) is not False
 
 
-def sa_forward(sa, xyz, feat):
-    """One PointnetSAModule in training mode: xyz (B,N,3) f32, feat (B,N,C) point-major (f32 | bf16) -> (new_xyz, (B,np,Cout) bf16)."""
+def sa_forward(sa, xyz, feat, ex=None):
+    """One PointnetSAModule in training mode: xyz (B,N,3) f32, feat (B,N,C) point-major (f32 | bf16) -> (new_xyz, (B,np,Cout) bf16).
+    ex: the StatExchange of SyncBatchNorm layers, or None."""
     from . import pointnet2_utils
     from .pointnet2 import _ext
     B, N, _ = xyz.shape
@@ -166,18 +312,23 @@ def sa_forward(sa, xyz, feat):
     for j in range(len(sa.mlp_spec) - 1):
         layer = getattr(mlp, f"layer{j}")
         bn = layer.bn.bn
-        X, stats = _ConvBNReLUFn.apply(X, layer.conv.weight, bn.weight, bn.bias, bn.eps)
+        X, stats = _ConvBNReLUFn.apply(X, layer.conv.weight, bn.weight, bn.bias, bn.eps, ex)
         _update_running_stats(bn, stats)
     out = _RowGroupMaxFn.apply(X, ns)           # (B*np, Cout)
     return new_xyz, out.view(B, np_, -1)
 
 
-def forward(net, pc):
-    """PointNetPP.forward for a trainable backbone: (n, P, 3 + C) f32 -> (n, D)."""
+def forward(net, pc, exchange=None):
+    """PointNetPP.forward for a trainable backbone: (n, P, 3 + C) f32 -> (n, D).  exchange: the StatExchange of the
+    SyncBatchNorm layers; by default exchange_for(net, pc.device)."""
     from . import ops
+    ex = exchange if exchange is not None else exchange_for(net, pc.device)
+    if ex is False:
+        raise RuntimeError("the SyncBatchNorm statistics exchange is unavailable; pn_train.available() routes such a net to "
+                           "PointNetPP.forward_generic")
     xyz = pc[..., 0:3].contiguous()
     feat = pc[..., 3:].contiguous() if pc.size(-1) > 3 else None
     for sa in net.encoder:
-        new_xyz, feat = sa_forward(sa, xyz, feat)
+        new_xyz, feat = sa_forward(sa, xyz, feat, ex)
         xyz = new_xyz if new_xyz is not None else xyz
     return ops.linear(feat.reshape(feat.shape[0], -1), net.fc.weight, net.fc.bias)

@@ -516,25 +516,50 @@ class ObjClsStep:
     PointNet++ TRAINABLE with train-mode BatchNorm -> dropout -> 607-way open-vocabulary logits -> label-smoothed CE ->
     AdamW.  The point operators and their gradients (group_points_grad / gather) are the native kernels; conv / BatchNorm
     statistics run on cuDNN / ATen (the fused tensor-core SA-MLP is the eval-BN form).  cuda_graph=True captures the whole
-    step after three eager ones."""
+    step after three eager ones.
+
+    num_gpu > 1 (one process per GPU, process group initialised): the backbone's BatchNorm layers are SyncBatchNorm
+    (objcls.py:33-34).  Every rank starts from rank 0's parameters and buffers.  With cuda_graph=True and the native statistics
+    exchange available (pn_train.exchange_for) a step is graph A (forward + backward into one flat gradient buffer, the 18
+    SyncBatchNorm exchanges included) | one NCCL all-reduce (mean) of that buffer | graph B (AdamW), as PretrainStep's
+    data-parallel graph path; no collective is captured.  Otherwise the model runs eagerly under DDP."""
 
     def __init__(self, device, text_embeds, lr=1e-3, dtype=torch.bfloat16, seed=0, cuda_graph=False, num_gpu=1):
         torch.manual_seed(seed)
         self.device, self.dtype = torch.device(device), dtype
         self.model = M.ObjCls({"num_gpu": num_gpu, "solver": {"lr": lr}}, text_embeds=text_embeds).to(self.device).train()
         self.graph_mode = bool(cuda_graph) and self.device.type == "cuda"
+        self.ddp = self.flat_grads = self.graph_opt = None
+        if num_gpu > 1 and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            from . import pn_train
+            sync_module_state(self.model)
+            if self.graph_mode and pn_train.exchange_for(self.model.point_feature_extractor, self.device):
+                self.flat_grads = FlatGrads(self.model.parameters())
+            else:
+                self.graph_mode = False
+                self.ddp = nn.parallel.DistributedDataParallel(
+                    self.model, device_ids=[self.device.index] if self.device.type == "cuda" else None)
         self.optimizer = torch.optim.AdamW(self.model.parameters(), lr=torch.tensor(lr, device=self.device) if self.graph_mode else lr,
                                            fused=self.device.type == "cuda", capturable=self.graph_mode)
         self.graph = self.static_batch = self.static_loss = None
 
-    def _raw(self, batch):
-        self.optimizer.zero_grad(set_to_none=False)
+    def _fwd_bwd(self, batch):
+        if self.flat_grads is not None:
+            self.flat_grads.zero()
+        else:
+            self.optimizer.zero_grad(set_to_none=False)
         with torch.autocast(self.device.type, dtype=self.dtype, enabled=self.dtype != torch.float32):
-            out = self.model(dict(batch))
+            out = (self.ddp if self.ddp is not None else self.model)(dict(batch))
             loss = L.obj_cls_loss(out)
         loss.backward()
-        self.optimizer.step()
         return loss.detach()
+
+    def _raw(self, batch):
+        loss = self._fwd_bwd(batch)
+        if self.flat_grads is not None:
+            self.flat_grads.all_reduce_mean()
+        self.optimizer.step()
+        return loss
 
     def step(self, batch):
         if not self.graph_mode:
@@ -552,11 +577,21 @@ class ObjClsStep:
             from . import _lib
             n0 = _lib.launch_count()
             self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
-                self.static_loss = self._raw(self.static_batch)
+            if self.flat_grads is None:
+                with torch.cuda.graph(self.graph):
+                    self.static_loss = self._raw(self.static_batch)
+            else:
+                with torch.cuda.graph(self.graph):
+                    self.static_loss = self._fwd_bwd(self.static_batch)
+                self.graph_opt = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(self.graph_opt, pool=self.graph.pool()):
+                    self.optimizer.step()
             self.native_launches_per_step = _lib.launch_count() - n0
         for k, dst in self.static_batch.items():
             if batch[k].data_ptr() != dst.data_ptr():
                 dst.copy_(batch[k], non_blocking=True)
         self.graph.replay()
+        if self.graph_opt is not None:
+            self.flat_grads.all_reduce_mean()
+            self.graph_opt.replay()
         return self.static_loss
