@@ -197,6 +197,32 @@ int sv_cross_entropy_fwd_bwd_strided(const void *logits, long long row_stride, i
                                      int V, long long ignore_index, float *loss_rows, void *grad_logits,
                                      long long grad_row_stride, void *stream);
 
+/* Binary cross-entropy with logits, forward + gradient in one launch (reference: optim/loss/loss.py:50-53 `answer_loss`, and
+ * the ScanQA form of optim/loss/contra_loss.py:33-34 — F.binary_cross_entropy_with_logits(x, y.float(), weight=w,
+ * reduction='sum') / R).  logits (R, row_stride >= C) bf16 (is_bf16 = 1) or f32, columns [0, C) used; labels (R, C) int64
+ * contiguous; weight (R, C) bytes (bool: nonzero = 1) or NULL.
+ * loss_rows[r] = sum_c w (max(x,0) - x y + log1p(exp(-|x|)));  *loss_out = (sum_r loss_rows[r]) / R, the rows added in a fixed
+ * order (bitwise reproducible).  counter: a zero-initialised device word, left at zero on completion (one per stream).
+ * grad_logits (may be NULL): w (sigmoid(x) - y), same dtype, rows grad_row_stride (>= C) elements apart, columns
+ * [C, grad_row_stride) written as zeros — NOT yet scaled by dL/dloss / R (sv_scale_inplace does that in the backward). */
+int sv_bce_logits_fwd_bwd(const void *logits, long long row_stride, int is_bf16, const long long *labels,
+                          const unsigned char *weight, int R, int C, float *loss_rows, float *loss_out, unsigned *counter,
+                          void *grad_logits, long long grad_row_stride, void *stream);
+
+/* Masked soft-attention pooling of one glimpse (reference: modules/heads/qa_head.py:42-70 AttFlat with flat_glimpses = 1).
+ * score: the (B*L, score_rs) bf16 output of the N = 1 score linear (column 0 used; score_rs = 8 for the padded rows of the
+ * native linear); x (B, L, D) bf16 with batch stride x_bs and row stride x_rs (elements, % 8 == 0, 16-byte aligned base),
+ * D % 8 == 0; pad_mask (B, L) bytes, nonzero = masked (may be NULL); 1 <= L <= 8192.
+ * forward:  s = pad_mask ? -1e9 : score (exactly the reference's fp32 fill: a fully masked row gets weights 1/L);
+ *           p (B, L) f32 = softmax over L of s (saved for the backward); pooled (B, D) bf16 = sum_l p_l x_l (fp32 accumulation).
+ * backward: dpooled (B, D) bf16, row stride dp_rs; dx (B, L, D) bf16 contiguous = p_l dpooled;
+ *           dscore (B*L, score_rs) bf16: column 0 = p_l (<dpooled, x_l> - sum_l' p_l' <dpooled, x_l'>), 0 at masked positions,
+ *           columns 1.. zero — the padded gradient the score linear's backward reads. */
+int sv_attn_pool_fwd(const void *score, int score_rs, const void *x, long long x_bs, int x_rs, const unsigned char *pad_mask,
+                     int B, int L, int D, float *p, void *pooled, void *stream);
+int sv_attn_pool_bwd(const void *dpooled, int dp_rs, const float *p, const void *x, long long x_bs, int x_rs,
+                     const unsigned char *pad_mask, int B, int L, int D, void *dx, void *dscore, int score_rs, void *stream);
+
 /* Backward of a stand-alone activation behind a linear layer (the FFN form fuses this into sv_linear_dgrad_bf16):
  * out = g x act'(.), (M,N) bf16, N % 8 == 0.  mode 1: relu, aux = forward output; mode 2: gelu(erf), aux = pre-activation. */
 int sv_act_bwd_bf16(const void *g, int ldg, const void *aux, int ld_aux, int mode, int M, int N, void *out, int ldo,

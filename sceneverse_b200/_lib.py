@@ -121,6 +121,12 @@ _GPS_SIGS = {
     "sv_embedding_bwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, ctypes.c_longlong, ctypes.c_longlong,
                          c_void_p, c_void_p],
     "sv_scale_inplace": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p],
+    "sv_bce_logits_fwd_bwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                              c_void_p, c_void_p, ctypes.c_longlong, c_void_p],
+    "sv_attn_pool_fwd": [c_void_p, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
+                         c_void_p, c_void_p],
+    "sv_attn_pool_bwd": [c_void_p, c_int, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, c_int,
+                         c_void_p, c_void_p, c_int, c_void_p],
     "sv_adamw_scratch_floats": [],
     "sv_adamw_flat": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_int, c_float, c_void_p,
                       c_void_p, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p],

@@ -141,6 +141,8 @@ class OpenVocab(nn.Module):
             txt_cls, obj_cls_post, obj_cls_pre, og3d = self.ground_head(lang_f, obj_f, obj_pre, data_dict['obj_masks'])
             data_dict.update(txt_cls_logits=txt_cls, obj_cls_post_logits=obj_cls_post, obj_cls_pre_logits=obj_cls_pre,
                              og3d_logits=og3d)
+        if getattr(self, "qa_head", None) is not None:
+            data_dict['answer_scores'] = self.qa_head(obj_f, data_dict['obj_masks'], lang_f, data_dict['txt_masks'])
         if getattr(self, "pretrain_head", None) is not None:
             output = self.pretrain_head(lang_f, obj_f)
             if isinstance(output, tuple):
@@ -156,7 +158,7 @@ class OpenVocab(nn.Module):
         groups += no_decay_param_group(self.lang_encoder.named_parameters(), lr_of(self.cfg.model.language))
         groups += no_decay_param_group(self.point_encoder.named_parameters(), lr_of(self.cfg.model.vision))
         groups += no_decay_param_group(self.unified_encoder.named_parameters(), lr_of(self.cfg.model.grounding))
-        for head in ("ground_head", "pretrain_head"):
+        for head in ("ground_head", "qa_head", "pretrain_head"):
             if head in self.head_list:
                 groups += no_decay_param_group(getattr(self, head).named_parameters(),
                                                lr_of(getattr(self.cfg.model.heads, head)))
@@ -209,6 +211,33 @@ def scanrefer_config(num_gpu=1, text_features=None):
     cfg["model"]["loss_list"] = ["og3d_loss"]
     cfg["model"]["vis_loss_list"] = ["og3d_loss"]
     return cfg
+
+
+def _qa_config(num_gpu, text_features, task, num_answers, losses):
+    cfg = pretrain_config(num_gpu, text_features=text_features)
+    cfg["task"] = task
+    cfg["data"]["args"]["use_scene_cap"] = False
+    cfg["solver"]["lr"] = 1e-4
+    cfg["solver"]["sched"] = {"name": "warmup_cosine", "args": {"warmup_steps": 5000}}
+    cfg["model"]["heads"] = {"head_list": ["qa_head"],
+                             "qa_head": {"name": "QAHeadV1",
+                                         "args": {"hidden_size": 768, "mlp_size": 256, "glimpse": 1, "flat_out_size": 512,
+                                                  "num_answers": num_answers}}}
+    cfg["model"]["loss_list"] = list(losses)
+    cfg["model"]["vis_loss_list"] = list(losses)
+    return cfg
+
+
+def scanqa_config(num_gpu=1, text_features=None):
+    """configs/final/finetune/scanqa_finetune.yaml: the pre-training encoders (frozen backbone, inter 'before', no scene
+    captions), QAHeadV1 over 8864 answers, `answer_loss` + the masked-BCE TextObjWithinBatch of task 'ScanQA'; lr 1e-4
+    (language 1e-5, vision and grounding 1e-4), grad_norm 5.0, betas (0.9, 0.98), 5000 warm-up steps."""
+    return _qa_config(num_gpu, text_features, "ScanQA", 8864, ["answer_loss", "TextObjWithinBatch"])
+
+
+def sqa3d_config(num_gpu=1, text_features=None):
+    """configs/final/finetune/sqa3d_finetune.yaml: as scanqa_config with task 'SQA3D', 706 answers and `answer_loss` only."""
+    return _qa_config(num_gpu, text_features, "SQA3D", 706, ["answer_loss"])
 
 
 def warmup_cosine(step, warmup_step, total_step, minimum_ratio=1e-5):

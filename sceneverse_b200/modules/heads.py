@@ -93,7 +93,8 @@ class _AttentionPool(nn.Module):
     """Masked soft-attention pooling over a token axis followed by a merge projection (reference: qa_head.py:42-70;
     parameter names `mlp.fc.linear.*`, `mlp.linear.*`, `linear_merge.*` kept for checkpoint compatibility).  One score
     MLP (hidden -> mid -> glimpses, GELU + dropout), scores of masked tokens set to -1e9 before the softmax over tokens;
-    the glimpse-weighted sums are one batched contraction instead of the reference's per-glimpse loop + cat."""
+    the glimpse-weighted sums are one batched contraction instead of the reference's per-glimpse loop + cat (ops.attention_pool:
+    one native kernel per direction for one glimpse, reading the padded score rows of the N = 1 linear in place)."""
 
     def __init__(self, hidden_size, mid_size=512, glimpses=1, out_size=1024, pdrop=0.1):
         super().__init__()
@@ -108,11 +109,8 @@ class _AttentionPool(nn.Module):
         h = ops.linear(x, self.mlp.fc.linear.weight, self.mlp.fc.linear.bias, activation="gelu")
         if self.pdrop > 0:
             h = nn.functional.dropout(h, self.pdrop, self.training)
-        att = ops.linear(h, self.mlp.linear.weight, self.mlp.linear.bias)            # (B, L, G)
-        if pad_mask is not None:
-            att = att.masked_fill(pad_mask.unsqueeze(2), -1e9)
-        att = torch.softmax(att.float(), dim=1).to(x.dtype)
-        pooled = torch.einsum("blg,bld->bgd", att, x).flatten(1)                      # glimpse-major, like the cat
+        att = ops.padded_vocab_linear(h, self.mlp.linear.weight, self.mlp.linear.bias)   # (B, L, G), rows padded to 8
+        pooled = ops.attention_pool(att, x, pad_mask)                                   # (B, G*D), glimpse-major like the cat
         return ops.linear(pooled, self.linear_merge.weight, self.linear_merge.bias)
 
 
@@ -120,7 +118,9 @@ class _AttentionPool(nn.Module):
 class QAHeadV1(nn.Module):
     """ScanQA / SQA3D answer head (reference: modules/heads/qa_head.py:72-90): attention-pool the object and the text
     tokens, LayerNorm(sum), 2-layer GELU classifier over the answer vocabulary.  Same constructor, forward contract
-    (obj_embeds, obj_masks, txt_embeds, txt_masks; masks True = valid) and state_dict keys."""
+    (obj_embeds, obj_masks, txt_embeds, txt_masks; masks True = valid) and state_dict keys.  The classifier's first linear
+    carries the (erf) GELU in its epilogue; the answer layer writes rows padded to a multiple of 8 answers (SQA3D: 706 -> 712),
+    which ops.bce_with_logits_sum reads in place."""
 
     def __init__(self, cfg, hidden_size=768, mlp_size=256, glimpse=1, flat_out_size=512, num_answers=8864):
         super().__init__()
@@ -134,4 +134,6 @@ class QAHeadV1(nn.Module):
         object_feat = self.attflat_visual(obj_embeds, obj_masks.logical_not())
         lang_feat = self.attflat_lang(txt_embeds, txt_masks.logical_not())
         fuse = self.fusion_norm(lang_feat, residual=object_feat)
-        return self.answer_cls(fuse)
+        fc0, drop, fc3 = self.answer_cls[0], self.answer_cls[2], self.answer_cls[3]
+        h = drop(ops.linear(fuse, fc0.weight, fc0.bias, activation="gelu"))
+        return ops.padded_vocab_linear(h, fc3.weight, fc3.bias)

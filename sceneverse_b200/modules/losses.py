@@ -39,6 +39,12 @@ def lm_cls_loss(data_dict):
     return ops.cross_entropy(data_dict["txt_lm_cls_logits"], target, ignore_index=-1)
 
 
+def answer_loss(data_dict):
+    """loss.py:50-53: BCE with logits over the answer vocabulary against the multi-hot `answer_label` (int64, read as
+    float), summed and divided by the batch size; all-zero rows (unanswerable questions) still count."""
+    return ops.bce_with_logits_sum(data_dict["answer_scores"], data_dict["answer_label"])
+
+
 def obj_cls_loss(data_dict, smoothing=0.3):
     """optim/loss/loss.py:96-102 (ObjCls pre-training)."""
     ce = F.cross_entropy(data_dict["obj_logits"].permute(0, 2, 1), data_dict["obj_labels"], reduction='none',
@@ -50,16 +56,32 @@ def _num_gpu(cfg):
     return cfg["num_gpu"] if isinstance(cfg, dict) else cfg.num_gpu
 
 
+def _task(cfg):
+    return cfg.get("task") if isinstance(cfg, dict) else getattr(cfg, "task", None)
+
+
 @LOSS_REGISTRY.register()
 class TextObjWithinBatch(nn.Module):
+    """contra_loss.py:11-38.  Default: cross-entropy over the valid objects against one target id (B, 1).  task 'ScanQA':
+    masked BCE with logits over all object slots against a multi-hot (B, O) target (several objects, or the masked
+    'no target' placeholder slot), weight = obj_masks, summed and divided by B."""
+
     def __init__(self, cfg):
         super().__init__()
         self.distributed = _num_gpu(cfg) > 1
+        self.bce = _task(cfg) in ["ScanQA"]
 
     def forward(self, data_dict):
         obj_feats = ops.l2_normalize(data_dict["intra_obj_embeds"])
         text_feats = ops.l2_normalize(data_dict["intra_text_embed"])
         logits = torch.einsum("bod,bd->bo", obj_feats, text_feats)
+        if self.bce:
+            labels = data_dict["tgt_object_id"]
+            if labels.dim() != 2 or labels.shape != logits.shape:
+                raise ValueError(f"TextObjWithinBatch(task='ScanQA') needs a multi-hot tgt_object_id of shape (B, O) = "
+                                 f"{tuple(logits.shape)}, got {tuple(labels.shape)} (a (B, 1) target id is the "
+                                 "cross-entropy form of the other tasks)")
+            return ops.bce_with_logits_sum(logits, labels, weight=data_dict["obj_masks"])
         logits = logits.masked_fill(data_dict["obj_masks"].logical_not(), -float('inf'))
         return F.cross_entropy(logits, data_dict["tgt_object_id"].squeeze(-1))
 
@@ -113,9 +135,10 @@ class TextSceneBetweenBatch(_SymmetricInfoNCE):
 
 
 class Loss(nn.Module):
-    """optim/loss/loss.py:111-148 list-loss container (cfg.model.loss_list / vis_loss_list)."""
+    """optim/loss/loss.py:111-148 list-loss container (cfg.model.loss_list / vis_loss_list); `task` (cfg.task) reaches the
+    registry losses' cfg (TextObjWithinBatch switches to its BCE form for 'ScanQA')."""
 
-    def __init__(self, loss_list, vis_loss_list=None, num_gpu=1, emulate_dist=False):
+    def __init__(self, loss_list, vis_loss_list=None, num_gpu=1, emulate_dist=False, task=None):
         super().__init__()
         self.selected_keys = list(loss_list)
         self.all_keys = list(dict.fromkeys(list(vis_loss_list or []) + self.selected_keys))
@@ -124,7 +147,7 @@ class Loss(nn.Module):
             if k in globals() and callable(globals()[k]) and not isinstance(globals()[k], type):
                 self.loss_fn[k] = globals()[k]
             else:
-                self.loss_fn[k] = LOSS_REGISTRY.get(k)({"num_gpu": num_gpu, "emulate_dist": emulate_dist})
+                self.loss_fn[k] = LOSS_REGISTRY.get(k)({"num_gpu": num_gpu, "emulate_dist": emulate_dist, "task": task})
                 setattr(self, k, self.loss_fn[k])
 
     def forward(self, data_dict):

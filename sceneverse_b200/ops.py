@@ -14,7 +14,9 @@ NATIVE = {"linear": True,               # every nn.Linear: native wgmma GEMM for
           "calc_pairwise_locs": True,
           "cross_entropy": True,        # masked-LM / grounding CE: fused native forward+gradient
           "layer_norm": True,           # dropout + residual add + LayerNorm: one native pass per direction
-          "l2_normalize": True}         # F.normalize of the contrastive heads: one native kernel per direction
+          "l2_normalize": True,         # F.normalize of the contrastive heads: one native kernel per direction
+          "bce_with_logits": True,      # QA answer loss / ScanQA within-batch loss: fused native forward+gradient
+          "attention_pool": True}       # AttFlat pooling of the QA head (one glimpse): one native kernel per direction
 
 
 _dropout_calls = [0]
@@ -595,6 +597,149 @@ class _CrossEntropyFn(torch.autograd.Function):
         return grad.mul_(scale.to(grad.dtype)), None, None, None
 
 
+_BCE_COUNTERS = {}
+
+
+def _bce_counter(device):
+    """The zero-initialised completion counter of sv_bce_logits_fwd_bwd on `device` (the kernel leaves it at zero)."""
+    c = _BCE_COUNTERS.get(device)
+    if c is None:
+        c = _BCE_COUNTERS[device] = torch.zeros(1, dtype=torch.int32, device=device)
+    return c
+
+
+class _BCEWithLogitsFn(torch.autograd.Function):
+    """sum of binary cross-entropy with logits over (R, C) divided by R; loss and gradient from ONE native launch.  n_classes <
+    logits.shape[1]: the trailing columns are padding (padded-vocabulary rows), ignored by the loss and zero in the gradient.
+    The backward scales the saved gradient in place, as _CrossEntropyFn does."""
+
+    @staticmethod
+    def forward(ctx, logits2d, labels2d, weight_u8, n_classes):
+        from . import _lib
+        R, W = logits2d.shape
+        dev = logits2d.device
+        loss_rows = torch.empty(R, dtype=torch.float32, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        grad = torch.empty((R, W), dtype=logits2d.dtype, device=dev) if logits2d.requires_grad else None
+        lib = _lib.gps()
+        with torch.cuda.device(dev):
+            st = lib.sv_bce_logits_fwd_bwd(
+                logits2d.data_ptr(), logits2d.stride(0), 1 if logits2d.dtype == torch.bfloat16 else 0, labels2d.data_ptr(),
+                weight_u8.data_ptr() if weight_u8 is not None else None, R, n_classes, loss_rows.data_ptr(), loss.data_ptr(),
+                _bce_counter(dev).data_ptr(), grad.data_ptr() if grad is not None else None, W,
+                torch.cuda.current_stream(dev).cuda_stream)
+        _lib.check(lib, st, "sv_bce_logits_fwd_bwd")
+        ctx.save_for_backward(grad)
+        ctx.rows, ctx.scaled = R, False
+        return loss
+
+    @staticmethod
+    def backward(ctx, gout):
+        (grad,) = ctx.saved_tensors
+        if ctx.scaled:
+            raise RuntimeError("ops.bce_with_logits_sum: backward through the same graph twice is not supported (the saved "
+                               "gradient buffer is consumed in place)")
+        ctx.scaled = True
+        scale = (gout.float() / ctx.rows).reshape(1).contiguous()
+        if grad.is_contiguous() and grad.numel() % 8 == 0 and grad.data_ptr() % 16 == 0:
+            from . import _lib
+            lib = _lib.gps()
+            with torch.cuda.device(grad.device):
+                st = lib.sv_scale_inplace(grad.data_ptr(), grad.numel(), 1 if grad.dtype == torch.bfloat16 else 0,
+                                          scale.data_ptr(), torch.cuda.current_stream(grad.device).cuda_stream)
+            _lib.check(lib, st, "sv_scale_inplace")
+            return grad, None, None, None
+        return grad.mul_(scale.to(grad.dtype)), None, None, None
+
+
+def bce_with_logits_sum(logits, labels, weight=None):
+    """F.binary_cross_entropy_with_logits(logits, labels.float(), weight=weight, reduction='sum') / logits.shape[0] for
+    (R, C) logits and labels (optim/loss/loss.py:50-53 `answer_loss`; the ScanQA form of TextObjWithinBatch,
+    contra_loss.py:33-34).  CUDA bf16 / f32 logits with int64 labels and a bool / uint8 weight: the fused native kernel,
+    reading a padded-vocabulary row (ops.padded_vocab_linear) in place and returning the gradient in that padded layout;
+    anything else: the torch formulation."""
+    if logits.dim() != 2 or labels.shape != logits.shape or (weight is not None and weight.shape != logits.shape):
+        raise ValueError(f"bce_with_logits_sum: logits {tuple(logits.shape)}, labels {tuple(labels.shape)} and weight "
+                         f"{None if weight is None else tuple(weight.shape)} must be the same (R, C)")
+    R, C = logits.shape
+    src = logits
+    padded = getattr(logits, "_sv_padded", None)
+    if padded is not None and padded.is_cuda and padded.dim() == 2 and padded.shape[0] == R and padded.is_contiguous():
+        src = padded
+    native = src.is_cuda and src.dtype in (torch.bfloat16, torch.float32) and src.stride(1) == 1 and R > 0 and C > 0 and \
+        labels.is_cuda and labels.dtype == torch.int64 and \
+        (weight is None or (weight.is_cuda and weight.dtype in (torch.bool, torch.uint8)))
+    if native:
+        w = None if weight is None else weight.contiguous().view(torch.uint8)
+        return _BCEWithLogitsFn.apply(src, labels.contiguous(), w, C)
+    return F.binary_cross_entropy_with_logits(logits, labels.float(), weight=weight, reduction='sum') / logits.shape[0]
+
+
+class _AttentionPoolFn(torch.autograd.Function):
+    """pooled = sum_l softmax_l(masked score) x_l for one glimpse (modules/heads/qa_head.py:57-69), one native launch per
+    direction.  `scores` is the PADDED (B, L, 8) output of the N = 1 score linear; its gradient is returned in that layout."""
+
+    @staticmethod
+    def forward(ctx, scores, x, pad_mask_u8):
+        from . import _lib
+        B, L, D = x.shape
+        p = torch.empty((B, L), dtype=torch.float32, device=x.device)
+        pooled = torch.empty((B, D), dtype=torch.bfloat16, device=x.device)
+        lib = _lib.gps()
+        with torch.cuda.device(x.device):
+            st = lib.sv_attn_pool_fwd(scores.data_ptr(), scores.shape[-1], x.data_ptr(), x.stride(0), x.stride(1),
+                                      pad_mask_u8.data_ptr() if pad_mask_u8 is not None else None, B, L, D, p.data_ptr(),
+                                      pooled.data_ptr(), torch.cuda.current_stream(x.device).cuda_stream)
+        _lib.check(lib, st, "sv_attn_pool_fwd")
+        ctx.save_for_backward(x, p, pad_mask_u8)
+        ctx.score_w = scores.shape[-1]
+        return pooled
+
+    @staticmethod
+    def backward(ctx, g):
+        from . import _lib
+        x, p, mask = ctx.saved_tensors
+        B, L, D = x.shape
+        g = g.to(torch.bfloat16)
+        if g.stride(1) != 1 or g.stride(0) % 8 or g.data_ptr() % 16:
+            g = g.contiguous()
+        dx = torch.empty((B, L, D), dtype=torch.bfloat16, device=x.device)
+        dscore = torch.empty((B, L, ctx.score_w), dtype=torch.bfloat16, device=x.device)
+        lib = _lib.gps()
+        with torch.cuda.device(x.device):
+            st = lib.sv_attn_pool_bwd(g.data_ptr(), g.stride(0), p.data_ptr(), x.data_ptr(), x.stride(0), x.stride(1),
+                                      mask.data_ptr() if mask is not None else None, B, L, D, dx.data_ptr(), dscore.data_ptr(),
+                                      ctx.score_w, torch.cuda.current_stream(x.device).cuda_stream)
+        _lib.check(lib, st, "sv_attn_pool_bwd")
+        return dscore, dx, None
+
+
+def _attention_pool_torch(att, x, pad_mask):
+    if pad_mask is not None:
+        att = att.masked_fill(pad_mask.unsqueeze(2), -1e9)
+    att = torch.softmax(att.float(), dim=1).to(x.dtype)
+    return torch.einsum("blg,bld->bgd", att, x).flatten(1)                      # glimpse-major, like the reference's cat
+
+
+def attention_pool(scores, x, pad_mask=None):
+    """AttFlat's pooling (modules/heads/qa_head.py:57-69): scores (B, L, G) of the score MLP, x (B, L, D) tokens, pad_mask
+    (B, L) bool, True = padding -> (B, G*D), the softmax over L in fp32 with masked scores set to -1e9.  CUDA under bf16 with
+    G = 1 and scores from ops.padded_vocab_linear (the padded parent is read in place): one native kernel per direction;
+    otherwise (CPU, the fp32 parity path, G > 1, shapes the kernels reject) the torch formulation."""
+    padded = getattr(scores, "_sv_padded", None)
+    B, L, D = x.shape
+    if padded is not None and scores.shape[-1] == 1 and padded.dim() == 3 and padded.shape[:2] == (B, L) and \
+            padded.is_contiguous() and padded.dtype == torch.bfloat16 and x.is_cuda and D % 8 == 0 and 1 <= L <= 8192 and \
+            B > 0 and (x.dtype == torch.bfloat16 or (_autocast_on() and x.dtype == torch.float32)) and \
+            (pad_mask is None or (pad_mask.is_cuda and pad_mask.dtype == torch.bool and pad_mask.shape == (B, L))):
+        xb = x if x.dtype == torch.bfloat16 else x.to(torch.bfloat16)
+        if xb.stride(2) != 1 or xb.stride(1) % 8 or xb.stride(0) % 8 or xb.data_ptr() % 16:
+            xb = xb.contiguous()
+        m = None if pad_mask is None else pad_mask.contiguous().view(torch.uint8)
+        return _AttentionPoolFn.apply(padded, xb, m)
+    return _attention_pool_torch(scores, x, pad_mask)
+
+
 def padded_vocab_linear(h, weight, bias):
     """(..., K) -> (..., V) logits of a wide classifier (BERT LM head, modules/heads/pretrain_head.py:22-32: decoder + bias).
     On the native path the GEMM writes rows padded to a multiple of 8 classes (16-byte rows, pad columns zero); the returned
@@ -603,7 +748,11 @@ def padded_vocab_linear(h, weight, bias):
     V = weight.shape[0]
     if _native_linear_ok(h, weight):
         lp = _LinearFn.apply(h, weight, bias, None)
-        out = lp[..., :V] if lp.shape[-1] != V else lp
+        if lp.shape[-1] == V:
+            # no pad columns: nothing to carry (and `lp._sv_padded = lp` would be a reference cycle that keeps the whole
+            # autograd graph alive until the next garbage collection — fatal for a CUDA-graph capture that follows)
+            return lp
+        out = lp[..., :V]
         out._sv_padded = lp
         return out
     return linear(h, weight, bias)

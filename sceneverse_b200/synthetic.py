@@ -81,15 +81,17 @@ def adversarial_clouds(seed, N):
     return out
 
 
-def scene_batch(seed, B=64, O=80, P=1024, L=50, Ls=300, min_obj=8, all_valid=False):
+def scene_batch(seed, B=64, O=80, P=1024, L=50, Ls=300, min_obj=8, all_valid=False, max_obj=None):
     """Synthetic `data_dict` with the key set / dtypes of the reference's dataset wrappers
     (data/datasets/dataset_wrapper.py:38-111,147-195; SURVEY.md §8a row D), as numpy arrays:
     txt_ids/txt_masks (B,L) int64, obj_fts (B,O,P,6) f32 (padded objects all 1.0), obj_locs (B,O,6) f32 (pad 0),
     obj_masks/obj_sem_masks (B,O) bool, obj_labels (B,O) int64 (pad -100), tgt_object_id (B,1) int64,
-    masked_lm_labels (B,L) int64 (-1 = ignore), scene_txt_ids/scene_txt_masks (B,Ls) int64."""
+    masked_lm_labels (B,L) int64 (-1 = ignore), scene_txt_ids/scene_txt_masks (B,Ls) int64.
+    Each scene has between min_obj and max_obj (default O) valid objects."""
     rng = np.random.default_rng(seed)
     d = {}
-    n_obj = np.full(B, O) if all_valid else rng.integers(min(min_obj, O), O + 1, size=B)
+    hi = O if max_obj is None else max_obj
+    n_obj = np.full(B, O) if all_valid else rng.integers(min(min_obj, hi), hi + 1, size=B)
     obj_fts = np.ones((B, O, P, 6), np.float32)
     obj_locs = np.zeros((B, O, 6), np.float32)
     obj_masks = np.zeros((B, O), bool)
@@ -124,4 +126,33 @@ def scene_batch(seed, B=64, O=80, P=1024, L=50, Ls=300, min_obj=8, all_valid=Fal
     lm[pick] = d["txt_ids"][pick]
     d["masked_lm_labels"] = lm
     d["scene_txt_ids"], d["scene_txt_masks"] = text(Ls)
+    return d
+
+
+def qa_batch(seed, task="ScanQA", B=32, O=80, P=1024, L=50, Ls=300, num_answers=8864, min_obj=8, unanswerable=0.1,
+             placeholder=0.15, edge_rows=False):
+    """scene_batch + the question-answering targets of data/datasets/scannet_old.py:442-459, drawn from a separate RNG
+    stream (scene_batch's arrays for the same seed are unchanged):
+    answer_label (B, num_answers) int64 multi-hot with 1-3 answers, or all zero for an `unanswerable` fraction of the
+    questions (the ones `use_unanswer: True` keeps);
+    task 'ScanQA': tgt_object_id (B, O) int64 multi-hot over 1-3 valid objects, or, for a `placeholder` fraction, only the
+    'no target' slot n_obj, which obj_masks masks (every scene keeps at least one padded slot for it).
+    edge_rows=True: row 0 has no answer and row B-1 only the placeholder target."""
+    d = scene_batch(seed, B=B, O=O, P=P, L=L, Ls=Ls, min_obj=min_obj, max_obj=O - 1 if task == "ScanQA" else None)
+    rng = np.random.default_rng([seed, 0x51A])
+    ans = np.zeros((B, num_answers), np.int64)
+    for b in range(B):
+        if rng.random() >= unanswerable and not (edge_rows and b == 0):
+            ans[b, rng.choice(num_answers, size=int(rng.integers(1, 4)), replace=False)] = 1
+    d["answer_label"] = ans
+    if task == "ScanQA":
+        n_obj = d["obj_masks"].sum(1)
+        tgt = np.zeros((B, O), np.int64)
+        for b in range(B):
+            n = int(n_obj[b])
+            if rng.random() < placeholder or (edge_rows and b == B - 1):
+                tgt[b, n] = 1
+            else:
+                tgt[b, rng.choice(n, size=int(rng.integers(1, min(3, n) + 1)), replace=False)] = 1
+        d["tgt_object_id"] = tgt
     return d

@@ -26,7 +26,7 @@ class StepModule(nn.Module):
         self.model = M.OpenVocab(cfg)
         c = M.to_cfg(cfg)
         self.loss = L.Loss(c.model.loss_list, c.model.vis_loss_list, num_gpu=c.num_gpu,
-                           emulate_dist=bool(c.get("emulate_dist", False)))
+                           emulate_dist=bool(c.get("emulate_dist", False)), task=c.get("task"))
         for n, p in self.model.named_parameters():
             if n.startswith(STATIC_UNUSED):
                 p.requires_grad = False
