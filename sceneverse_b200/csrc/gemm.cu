@@ -237,103 +237,133 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       rk[0] = attn::drop_row_key(seed, (unsigned long long)(m0 + r_lo));
       rk[1] = attn::drop_row_key(seed, (unsigned long long)(m0 + r_lo + 8));
     }
+    // The operands the epilogue reads (bias, the saved activation of a dgrad) are loaded for JB column groups at once, before
+    // any arithmetic uses them, at indices clamped into the tensor instead of behind bounds branches: a load behind a branch
+    // cannot be issued early, so every one of them used to wait out its full latency.  Elements past the edge compute on the
+    // clamped values and are never stored.
+    constexpr int JB = 4;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = n0 + 8 * j + cq;
-      const bool c_ok = col < g.N, two = col + 1 < g.N;
-      float mx0 = -INFINITY, mx1 = -INFINITY;   // rowmax: this thread's two rows
+    for (int jc = 0; jc < BN / 8; jc += JB) {
+      float bv[2 * JB], xv[2 * JB][2];
+      if (EPI == EPI_FWD && g.bias != nullptr) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = m0 + r_lo + 8 * h;
-        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (EPI == EPI_FWD) {
-          if (g.bias != nullptr && c_ok) {
-            v0 += __ldg(g.bias + col);
-            if (two) v1 += __ldg(g.bias + col + 1);
-          }
-          if (g.out2 != nullptr && c_ok && row < g.M)
-            store_pair_bf16(reinterpret_cast<__nv_bfloat16 *>(g.out2) + (size_t)row * g.ldo + col, two, (g.ldo & 1) == 0, v0, v1);
-          if (g.act == 1) {
-            v0 = fmaxf(v0, 0.f);
-            v1 = fmaxf(v1, 0.f);
-          } else if (g.act == 2) {
-            v0 = gelu_erf(v0);
-            v1 = gelu_erf(v1);
-          }
-          if (g.t16) {
-            const uint32_t hh = attn::drop_pair_hash(rk[h], (uint32_t)col >> 1);
-            v0 = (hh & 0xFFFFu) >= g.t16 ? v0 * g.inv_keep : 0.f;
-            v1 = (hh >> 16) >= g.t16 ? v1 * g.inv_keep : 0.f;
-          }
-          if (g.rowmax == 16) {
-            mx0 = fmaxf(mx0, v0);
-            mx1 = fmaxf(mx1, v1);
-            continue;
-          }
-        } else if (EPI == EPI_DGRAD) {
-          if (g.act != 0 && c_ok && row < g.M) {
-            // multiply by the activation (+ dropout) derivative read from the saved forward tensor
-            const __nv_bfloat16 *ax = reinterpret_cast<const __nv_bfloat16 *>(g.aux) + (size_t)row * g.ld_aux + col;
-            const float x0 = __bfloat162float(ax[0]), x1 = two ? __bfloat162float(ax[1]) : 0.f;
-            if (g.act == 1) {
-              v0 = x0 > 0.f ? v0 * g.inv_keep : 0.f;
-              v1 = x1 > 0.f ? v1 * g.inv_keep : 0.f;
-            } else {
-              float m0_ = 1.f, m1_ = 1.f;
-              if (g.t16) {
-                const uint32_t hh = attn::drop_pair_hash(rk[h], (uint32_t)col >> 1);
-                m0_ = (hh & 0xFFFFu) >= g.t16 ? g.inv_keep : 0.f;
-                m1_ = (hh >> 16) >= g.t16 ? g.inv_keep : 0.f;
-              }
-              v0 *= gelu_grad(x0) * m0_;
-              v1 *= gelu_grad(x1) * m1_;
-            }
-          }
-        }
-        if (!c_ok || row >= g.M) continue;
-        if (EPI == EPI_WGRAD || g.out_f32) {
-          float *o = reinterpret_cast<float *>(g.out) + (size_t)row * g.ldo + col;
-          if (EPI == EPI_WGRAD && g.red_out) {
-            atomicAdd(o, v0);
-            if (two) atomicAdd(o + 1, v1);
-          } else {
-            const float *res = EPI == EPI_FWD ? reinterpret_cast<const float *>(g.residual) : nullptr;
-            if (res != nullptr) {
-              v0 += res[(size_t)row * g.ldo + col];
-              if (two) v1 += res[(size_t)row * g.ldo + col + 1];
-            }
-            o[0] = v0;
-            if (two) o[1] = v1;
-          }
-        } else {
-          const __nv_bfloat16 *res = EPI == EPI_FWD ? reinterpret_cast<const __nv_bfloat16 *>(g.residual) : nullptr;
-          if (res != nullptr) {
-            v0 += __bfloat162float(res[(size_t)row * g.ldo + col]);
-            if (two) v1 += __bfloat162float(res[(size_t)row * g.ldo + col + 1]);
-          }
-          store_pair_bf16(reinterpret_cast<__nv_bfloat16 *>(g.out) + (size_t)row * g.ldo + col, two, (g.ldo & 1) == 0, v0, v1);
+        for (int jj = 0; jj < JB; ++jj) {
+          const int col = n0 + 8 * (jc + jj) + cq;
+          bv[2 * jj] = __ldg(g.bias + min(col, g.N - 1));
+          bv[2 * jj + 1] = __ldg(g.bias + min(col + 1, g.N - 1));
         }
       }
-      if (EPI == EPI_FWD && g.rowmax == 16) {
-        // the 16 rows of a warp (r_lo and r_lo + 8 over the 8 lane quads) are one group of 16 consecutive rows = the 16
-        // points of one cloud: max over this thread's two rows, then over the lane quads
-        float a0 = mx0, a1 = mx1;
+      if (EPI == EPI_DGRAD && g.act != 0) {
+        const __nv_bfloat16 *ax = reinterpret_cast<const __nv_bfloat16 *>(g.aux);
 #pragma unroll
-        for (int o = 4; o < 32; o <<= 1) {
-          a0 = fmaxf(a0, __shfl_xor_sync(0xffffffffu, a0, o));
-          a1 = fmaxf(a1, __shfl_xor_sync(0xffffffffu, a1, o));
+        for (int jj = 0; jj < JB; ++jj) {
+          const int col = n0 + 8 * (jc + jj) + cq;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const size_t r = (size_t)min(m0 + r_lo + 8 * h, g.M - 1) * g.ld_aux;
+            xv[2 * jj + h][0] = __bfloat162float(ax[r + min(col, g.N - 1)]);
+            xv[2 * jj + h][1] = __bfloat162float(ax[r + min(col + 1, g.N - 1)]);
+          }
         }
-        const int grow0 = m0 + c * 64 + w * 16;   // first row of the group
-        if (lane < 4 && c_ok && grow0 < g.M) {
-          const size_t orow = (size_t)(grow0 >> 4);
-          if (g.out_f32) {
-            float *o = reinterpret_cast<float *>(g.out) + orow * g.ldo + col;
-            o[0] = a0;
-            if (two) o[1] = a1;
+      }
+#pragma unroll
+      for (int jj = 0; jj < JB; ++jj) {
+        const int j = jc + jj;
+        const int col = n0 + 8 * j + cq;
+        const bool c_ok = col < g.N, two = col + 1 < g.N;
+        float mx0 = -INFINITY, mx1 = -INFINITY;   // rowmax: this thread's two rows
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = m0 + r_lo + 8 * h;
+          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (EPI == EPI_FWD) {
+            if (g.bias != nullptr) {
+              v0 += bv[2 * jj];
+              v1 += bv[2 * jj + 1];
+            }
+            if (g.out2 != nullptr && c_ok && row < g.M)
+              store_pair_bf16(reinterpret_cast<__nv_bfloat16 *>(g.out2) + (size_t)row * g.ldo + col, two, (g.ldo & 1) == 0, v0, v1);
+            if (g.act == 1) {
+              v0 = fmaxf(v0, 0.f);
+              v1 = fmaxf(v1, 0.f);
+            } else if (g.act == 2) {
+              v0 = gelu_erf(v0);
+              v1 = gelu_erf(v1);
+            }
+            if (g.t16) {
+              const uint32_t hh = attn::drop_pair_hash(rk[h], (uint32_t)col >> 1);
+              v0 = (hh & 0xFFFFu) >= g.t16 ? v0 * g.inv_keep : 0.f;
+              v1 = (hh >> 16) >= g.t16 ? v1 * g.inv_keep : 0.f;
+            }
+            if (g.rowmax == 16) {
+              mx0 = fmaxf(mx0, v0);
+              mx1 = fmaxf(mx1, v1);
+              continue;
+            }
+          } else if (EPI == EPI_DGRAD) {
+            if (g.act != 0) {
+              // multiply by the activation (+ dropout) derivative read from the saved forward tensor
+              const float x0 = xv[2 * jj + h][0], x1 = xv[2 * jj + h][1];
+              if (g.act == 1) {
+                v0 = x0 > 0.f ? v0 * g.inv_keep : 0.f;
+                v1 = x1 > 0.f ? v1 * g.inv_keep : 0.f;
+              } else {
+                float m0_ = 1.f, m1_ = 1.f;
+                if (g.t16) {
+                  const uint32_t hh = attn::drop_pair_hash(rk[h], (uint32_t)col >> 1);
+                  m0_ = (hh & 0xFFFFu) >= g.t16 ? g.inv_keep : 0.f;
+                  m1_ = (hh >> 16) >= g.t16 ? g.inv_keep : 0.f;
+                }
+                v0 *= gelu_grad(x0) * m0_;
+                v1 *= gelu_grad(x1) * m1_;
+              }
+            }
+          }
+          if (!c_ok || row >= g.M) continue;
+          if (EPI == EPI_WGRAD || g.out_f32) {
+            float *o = reinterpret_cast<float *>(g.out) + (size_t)row * g.ldo + col;
+            if (EPI == EPI_WGRAD && g.red_out) {
+              atomicAdd(o, v0);
+              if (two) atomicAdd(o + 1, v1);
+            } else {
+              const float *res = EPI == EPI_FWD ? reinterpret_cast<const float *>(g.residual) : nullptr;
+              if (res != nullptr) {
+                v0 += res[(size_t)row * g.ldo + col];
+                if (two) v1 += res[(size_t)row * g.ldo + col + 1];
+              }
+              o[0] = v0;
+              if (two) o[1] = v1;
+            }
           } else {
-            __nv_bfloat16 *o = reinterpret_cast<__nv_bfloat16 *>(g.out) + orow * g.ldo + col;
-            o[0] = __float2bfloat16_rn(a0);
-            if (two) o[1] = __float2bfloat16_rn(a1);
+            const __nv_bfloat16 *res = EPI == EPI_FWD ? reinterpret_cast<const __nv_bfloat16 *>(g.residual) : nullptr;
+            if (res != nullptr) {
+              v0 += __bfloat162float(res[(size_t)row * g.ldo + col]);
+              if (two) v1 += __bfloat162float(res[(size_t)row * g.ldo + col + 1]);
+            }
+            store_pair_bf16(reinterpret_cast<__nv_bfloat16 *>(g.out) + (size_t)row * g.ldo + col, two, (g.ldo & 1) == 0, v0, v1);
+          }
+        }
+        if (EPI == EPI_FWD && g.rowmax == 16) {
+          // the 16 rows of a warp (r_lo and r_lo + 8 over the 8 lane quads) are one group of 16 consecutive rows = the 16
+          // points of one cloud: max over this thread's two rows, then over the lane quads
+          float a0 = mx0, a1 = mx1;
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            a0 = fmaxf(a0, __shfl_xor_sync(0xffffffffu, a0, o));
+            a1 = fmaxf(a1, __shfl_xor_sync(0xffffffffu, a1, o));
+          }
+          const int grow0 = m0 + c * 64 + w * 16;   // first row of the group
+          if (lane < 4 && c_ok && grow0 < g.M) {
+            const size_t orow = (size_t)(grow0 >> 4);
+            if (g.out_f32) {
+              float *o = reinterpret_cast<float *>(g.out) + orow * g.ldo + col;
+              o[0] = a0;
+              if (two) o[1] = a1;
+            } else {
+              __nv_bfloat16 *o = reinterpret_cast<__nv_bfloat16 *>(g.out) + orow * g.ldo + col;
+              o[0] = __float2bfloat16_rn(a0);
+              if (two) o[1] = __float2bfloat16_rn(a1);
+            }
           }
         }
       }
