@@ -57,7 +57,7 @@ int sv_gemm_force_ctas(int ctas);
 
 /* Profiling: while `buf` (device, [grid][16] int64) is non-null every GEMM launch writes, per CTA, the first consumer
  * warpgroup's {loop cycles, cycles waiting for operands, 0, k-steps issued, clock at start, at end, loop nanoseconds
- * (globaltimer)}. */
+ * (globaltimer), epilogue: 1 = staged in shared memory and written by TMA, 0 = per-element stores}. */
 int sv_gemm_profile(long long *buf);
 
 /* ---- the three GEMMs of a linear layer y = x W^T + b with their fused epilogues (same wgmma kernel family) --------

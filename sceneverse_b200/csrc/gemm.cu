@@ -11,14 +11,18 @@
 // mbarrier ring of up to 8 stages that keeps loading the next tiles while the consumers run an epilogue; either operand
 // may be stored transposed in memory ([K][rows]) and is then staged as 64-column slabs and read MN-major by wgmma —
 // the dgrad / wgrad forms of a linear layer need no transposed copy.  Out-of-bounds rows / columns / K are zero-filled
-// by TMA, the epilogue masks its stores.
+// by TMA.  The epilogue stages its results in shared memory, one 64-row x 128-byte box at a time, and writes each box with
+// one TMA store (WGRAD: TMA reduce-add), which clips it at the tensor edge and drains while the warpgroup goes on to the
+// next box or the next tile's main loop; the last columns of a row that does not end on a 16-byte unit are copied out of the
+// box per element.  Outputs that cannot take such boxes (the SA3 row max, the residual add, pitches that are not whole
+// 16-byte units) keep per-element stores masked at the edge (template parameter OUT_TMA).
 //
 // Epilogue families (template parameter EPI):
 //   EPI_FWD   + bias -> (store pre-activation copy) -> relu | gelu(erf) -> dropout (counter hash, nothing stored)
 //             -> + residual -> bf16 | f32 store, or max over 16-row groups (PointNet++ SA3 neighbourhood max)
 //   EPI_DGRAD x activation derivative: relu+dropout from the saved forward OUTPUT (h > 0 ? 1/keep : 0), or gelu' from the
 //             saved pre-activation with the dropout mask regenerated from (seed, row, column)
-//   EPI_WGRAD fp32 result, split-K over the work list, atomic adds straight into the (flat) gradient buffer; the bias
+//   EPI_WGRAD fp32 result, split-K over the work list, reduce-adds into the (flat) gradient buffer; the bias
 //             gradient (column sums of dL/dy) comes out of the SAME main loop: one extra N = 8 wgmma per K step against a
 //             constant tile of ones (first column-tile only)
 #include <cstdio>
@@ -62,6 +66,7 @@ struct GemmArgs {
   int splits;               // split-K factor (>= 1); > 1 only with red_out
   int red_out;              // WGRAD: accumulate into out with atomic adds instead of storing
   float *bias_grad;         // WGRAD: [M] += row sums of A (the bias gradient), or null
+  int n_tma;                // OUT_TMA: columns [0, n_tma) go out by TMA, the rest of [0, N) per element (see run_gemm)
 };
 
 // Phi(x) = 0.5 (1 + erf(x / sqrt 2)) and e = exp(-x^2 / 2) with two MUFU ops: erf by Abramowitz-Stegun 7.1.26
@@ -96,14 +101,46 @@ __device__ __forceinline__ void store_pair_bf16(__nv_bfloat16 *o, bool two, bool
   }
 }
 
-template <int BN>
+// A staged output box: 64 rows (one consumer warpgroup's share of the tile) x 128 bytes (64 bf16 or 32 fp32 columns),
+// SWIZZLE_128B.  Each consumer warpgroup owns a ring of two, so one box can be written while the previous one drains.
+constexpr int OUT_BOX = 64 * 128;
+constexpr int OUT_RING = 2 * OUT_BOX;
+constexpr int SMEM_OPTIN = 232448;   // 227 KB: the sm_90 per-block opt-in limit
+
+template <int BN, int OUT_TMA>
 struct GemmCfg {
   static constexpr int A_STAGE = BM * BK * 2, B_STAGE = BN * BK * 2;
-  static constexpr int STAGES_RAW = (200 * 1024) / (A_STAGE + B_STAGE);
+  static constexpr int OUT = OUT_TMA ? 2 * OUT_RING : 0;   // the output rings of the two consumer warpgroups
+  // OUT_TMA: operand stages fill what is left after the output rings, 1 KB alignment slack, the 1 KB tile of ones (WGRAD
+  // bias-gradient operand) and the barriers of at most 8 stages.  The per-element kernels keep their 200 KB operand budget.
+  static constexpr int STAGES_RAW =
+      OUT_TMA ? (SMEM_OPTIN - OUT - 1024 - 1024 - 2 * 8 * 8) / (A_STAGE + B_STAGE) : (200 * 1024) / (A_STAGE + B_STAGE);
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  // + 1 KB alignment slack, 1 KB tile of ones (WGRAD bias-gradient operand), the barriers
-  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + 1024 + 1024 + 2 * STAGES * 8;
+  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + OUT + 1024 + 1024 + 2 * STAGES * 8;
+  static_assert(SMEM <= SMEM_OPTIN, "gemm_kernel shared memory exceeds the opt-in limit");
 };
+
+// Columns [n_tma, N) of a staged box (64 rows from row cm, 8 box_j columns from column cn): they lie past the last whole
+// 16-byte unit of a row, and a TMA store clips only to whole units, so they are copied out per element, from the box after
+// the warpgroup barrier that completed it.  out2 comes from the box at `pre` (ring slot 0).
+__device__ __forceinline__ void store_tail(const uint8_t *box, const uint8_t *pre, const GemmArgs &g, bool red, bool f32,
+                                           int cn, int cm, int t) {
+  const int r = t >> 1, row = cm + r;   // two threads per box row, alternate columns
+  if (row >= g.M) return;
+  const int sh = f32 ? 2 : 1;           // log2 of the element size
+  const int end = min(g.N - cn, 128 >> sh);
+  for (int cc = max(g.n_tma - cn, 0) + (t & 1); cc < end; cc += 2) {
+    const int byte = cc << sh;
+    const int off = r * 128 + ((((byte >> 4) ^ (r & 7)) << 4) | (byte & 15));
+    const size_t o = (size_t)row * g.ldo + cn + cc;
+    if (red) atomicAdd(reinterpret_cast<float *>(g.out) + o, *reinterpret_cast<const float *>(box + off));
+    else if (f32) reinterpret_cast<float *>(g.out)[o] = *reinterpret_cast<const float *>(box + off);
+    else {
+      reinterpret_cast<uint16_t *>(g.out)[o] = *reinterpret_cast<const uint16_t *>(box + off);
+      if (g.out2 != nullptr) reinterpret_cast<uint16_t *>(g.out2)[o] = *reinterpret_cast<const uint16_t *>(pre + off);
+    }
+  }
+}
 
 template <int BN, int TA, int TB>
 __device__ __forceinline__ void mma(float (&d)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -112,16 +149,20 @@ __device__ __forceinline__ void mma(float (&d)[BN / 2], uint64_t da, uint64_t db
   else wgmma_n192<TA, TB>(d, da, db, scale_d);
 }
 
-template <int BN, int EPI, int TA, int TB>
+// OUT_TMA = 1: the epilogue stages out (and out2) in shared memory and writes them by TMA store (WGRAD: TMA reduce-add)
+// through mapO / mapO2; 0: per-element stores (the maps are unused)
+template <int BN, int EPI, int TA, int TB, int OUT_TMA>
 __global__ void __launch_bounds__(NTHREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GemmArgs g) {
+gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+            const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapO2, const GemmArgs g) {
   extern __shared__ uint8_t smem_raw[];
-  using Cfg = GemmCfg<BN>;
+  using Cfg = GemmCfg<BN, OUT_TMA>;
   constexpr int A_STAGE = Cfg::A_STAGE, B_STAGE = Cfg::B_STAGE, STAGES = Cfg::STAGES;
   uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B tiles: 1024-byte aligned
   uint8_t *sA = smem;
   uint8_t *sB = smem + STAGES * A_STAGE;
-  uint8_t *sOnes = sB + STAGES * B_STAGE;                      // [8][64] bf16 ones (1 KB), WGRAD bias-gradient operand
+  uint8_t *sOut = sB + STAGES * B_STAGE;                       // [2 consumer warpgroups][OUT_RING] staged output boxes
+  uint8_t *sOnes = sOut + Cfg::OUT;                            // [8][64] bf16 ones (1 KB), WGRAD bias-gradient operand
   uint64_t *full = reinterpret_cast<uint64_t *>(sOnes + 1024);
   uint64_t *empty = full + STAGES;
 
@@ -193,6 +234,16 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   const uint32_t a_lbo = TA ? BK * 128 : 16, b_lbo = TB ? BK * 128 : 16;
   const uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
   const unsigned long long seed = (EPI != EPI_WGRAD && g.t16) ? attn::effective_seed(g.seed, g.seed_offset) : 0ull;
+  // staged output: a box holds box_j 8-column groups.  Without out2, box k of this warpgroup goes to ring slot k % 2; with
+  // out2, every box step fills both slots (slot 0 the pre-activation, slot 1 the output).
+  constexpr bool tma_out = OUT_TMA != 0;
+  const bool f32_out = EPI == EPI_WGRAD || g.out_f32;
+  const int box_j = f32_out ? 4 : 8;
+  const uint32_t ring = smem_u32(sOut) + (uint32_t)c * OUT_RING;
+  // this lane's byte offsets inside a box: stmatrix row addresses (bf16), or its two fp32 columns of row r_lo - 64 c
+  const uint32_t sm_row = (uint32_t)(w * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * 128u, sm_x = lane & 7, sm_j = lane >> 4;
+  const uint32_t f_row = (uint32_t)(w * 16 + (lane >> 2)) * 128u, f_hi = (lane >> 1) & 1, f_x = lane >> 2, f_lo = (lane & 1) * 8u;
+  uint32_t nbox = 0;
   uint32_t s = 0, ph = 0;
   long long p_full = 0, p_t0 = g.prof ? clock64() : 0, nks = 0;
   unsigned long long p_ns0 = 0;
@@ -244,7 +295,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     constexpr int JB = 4;
 #pragma unroll
     for (int jc = 0; jc < BN / 8; jc += JB) {
+      // boxes that start at or past N are not staged, so the box holding column N - 1 is the last one of the tile
+      if (tma_out && n0 + 8 * (jc - jc % box_j) >= g.N) break;
+      if (tma_out && jc % box_j == 0) {
+        // the slot(s) this box is staged in must have been read out by the TMA store that last used them
+        if (t == 0) {
+          if (g.out2 != nullptr) bulk_wait_read<0>();
+          else bulk_wait_read<1>();
+        }
+        wg_sync(1 + c);
+      }
       float bv[2 * JB], xv[2 * JB][2];
+      uint32_t pre[2 * JB];   // tma_out with out2: the packed bf16 pre-activation of (jj, h)
       if (EPI == EPI_FWD && g.bias != nullptr) {
 #pragma unroll
         for (int jj = 0; jj < JB; ++jj) {
@@ -281,8 +343,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
               v0 += bv[2 * jj];
               v1 += bv[2 * jj + 1];
             }
-            if (g.out2 != nullptr && c_ok && row < g.M)
-              store_pair_bf16(reinterpret_cast<__nv_bfloat16 *>(g.out2) + (size_t)row * g.ldo + col, two, (g.ldo & 1) == 0, v0, v1);
+            if (g.out2 != nullptr) {
+              if (tma_out) pre[2 * jj + h] = pack_bf16(v0, v1);
+              else if (c_ok && row < g.M)
+                store_pair_bf16(reinterpret_cast<__nv_bfloat16 *>(g.out2) + (size_t)row * g.ldo + col, two, (g.ldo & 1) == 0, v0, v1);
+            }
             if (g.act == 1) {
               v0 = fmaxf(v0, 0.f);
               v1 = fmaxf(v1, 0.f);
@@ -318,6 +383,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                 v1 *= gelu_grad(x1) * m1_;
               }
             }
+          }
+          if (tma_out) {   // staged below
+            acc[4 * j + 2 * h] = v0;
+            acc[4 * j + 2 * h + 1] = v1;
+            continue;
           }
           if (!c_ok || row >= g.M) continue;
           if (EPI == EPI_WGRAD || g.out_f32) {
@@ -367,6 +437,55 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
           }
         }
       }
+      if (tma_out) {
+        const uint32_t box = ring + (g.out2 != nullptr ? (uint32_t)OUT_BOX : (nbox & 1u) * OUT_BOX);
+        if (f32_out) {
+#pragma unroll
+          for (int jj = 0; jj < JB; ++jj) {
+            const int j = jc + jj;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t a = box + f_row + h * 1024u + ((((uint32_t)(2 * (j & 3)) + f_hi) ^ f_x) << 4) + f_lo;
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1])
+                           : "memory");
+            }
+          }
+        } else {
+          // columns 8 j .. 8 j + 15 of the warp's 16 rows are four 8x8 matrices: (h 0, j), (h 1, j), (h 0, j + 1), (h 1, j + 1)
+#pragma unroll
+          for (int jj = 0; jj < JB; jj += 2) {
+            const int j = jc + jj;
+            const uint32_t a = sm_row + (((((uint32_t)j + sm_j) & 7u) ^ sm_x) << 4);
+            stmatrix_x4(box + a, pack_bf16(acc[4 * j], acc[4 * j + 1]), pack_bf16(acc[4 * j + 2], acc[4 * j + 3]),
+                        pack_bf16(acc[4 * j + 4], acc[4 * j + 5]), pack_bf16(acc[4 * j + 6], acc[4 * j + 7]));
+            if (EPI == EPI_FWD && g.out2 != nullptr)
+              stmatrix_x4(ring + a, pre[2 * jj], pre[2 * jj + 1], pre[2 * jj + 2], pre[2 * jj + 3]);
+          }
+        }
+        if ((jc + JB) % box_j == 0) {
+          fence_proxy_async_smem();
+          wg_sync(1 + c);
+          const int cn = n0 + 8 * (jc + JB - box_j), cm = m0 + 64 * c;
+          if (t == 0) {
+            if (cn < g.n_tma && cm < g.M) {
+              if (EPI == EPI_WGRAD) {
+                tma_reduce_add_2d(&mapO, box, cn, cm);
+              } else {
+                tma_store_2d(&mapO, box, cn, cm);
+                if (g.out2 != nullptr) tma_store_2d(&mapO2, ring, cn, cm);
+              }
+            }
+            bulk_commit();
+          }
+          ++nbox;
+        }
+      }
+    }
+    if (tma_out && n0 + BN > g.n_tma && g.n_tma < g.N && m0 + 64 * c < g.M) {
+      // columns [n_tma, N) are in the last box staged (still intact: the next acquire comes after a barrier)
+      const int cn = n0 + ((g.N - 1 - n0) / (8 * box_j)) * 8 * box_j;
+      const uint32_t last = ring + (g.out2 != nullptr ? (uint32_t)OUT_BOX : ((nbox - 1) & 1u) * OUT_BOX);
+      store_tail(sOut + (last - smem_u32(sOut)), sOut + (ring - smem_u32(sOut)), g, EPI == EPI_WGRAD, f32_out, cn, m0 + 64 * c, t);
     }
     if (EPI == EPI_WGRAD && bias_tile && (lane & 3) == 0) {
       // every column of the N = 8 ones-product equals sum_k A[row][k]: the bias gradient of output feature `row`
@@ -374,12 +493,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       if (m0 + r_lo + 8 < g.M) atomicAdd(g.bias_grad + m0 + r_lo + 8, accb[2]);
     }
   }
-  if (g.prof && t == 0 && c == 0) {   // issue-loop cycles, of which waiting for operands, k-steps, start, end, ns
+  if (tma_out && t == 0) bulk_wait_all();   // the staged boxes must stay readable until the last store has read them
+  if (g.prof && t == 0 && c == 0) {   // issue-loop cycles, of which waiting for operands, k-steps, start, end, ns, epilogue
     long long *pp = g.prof + (size_t)blockIdx.x * 16;
     const long long t1 = clock64();
     unsigned long long ns1;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns1));
     pp[0] = t1 - p_t0; pp[1] = p_full; pp[2] = 0; pp[3] = nks; pp[4] = p_t0; pp[5] = t1; pp[6] = (long long)(ns1 - p_ns0);
+    pp[7] = OUT_TMA;
   }
 }
 
@@ -414,6 +535,22 @@ int make_map_mn(CUtensorMap *map, const void *ptr, int rows, int K, int ld) {
   return r == CUDA_SUCCESS ? SV_OK : SV_ERR_INVALID_ARG;
 }
 
+// row-major [rows, cols] output (bf16 or fp32) with leading dimension ld (elements): box = [64 rows x 128 bytes], the
+// staging layout of the epilogue.  TMA writes nothing outside [rows, cols].
+int make_out_map(CUtensorMap *map, void *ptr, int rows, int cols, int ld, bool f32) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) return SV_ERR_CUDA;
+  const int esz = f32 ? 4 : 2;
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esz), 64};
+  cuuint32_t es[2] = {1, 1};
+  CUresult r = fn(map, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, dims, strides, box,
+                  es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? SV_OK : SV_ERR_INVALID_ARG;
+}
+
 int device_sms(int *dev_out) {
   static int sms_of_dev[64] = {0};
   int dev = 0;
@@ -428,10 +565,11 @@ int device_sms(int *dev_out) {
   return sms_of_dev[dev];
 }
 
-template <int BN, int EPI, int TA, int TB>
-int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const GemmArgs &g, cudaStream_t st) {
-  constexpr size_t smem = GemmCfg<BN>::SMEM;
-  auto kern = gemm_kernel<BN, EPI, TA, TB>;
+template <int BN, int EPI, int TA, int TB, int OUT_TMA>
+int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mo, const CUtensorMap &mo2, const GemmArgs &g,
+                cudaStream_t st) {
+  constexpr size_t smem = GemmCfg<BN, OUT_TMA>::SMEM;
+  auto kern = gemm_kernel<BN, EPI, TA, TB, OUT_TMA>;
   static bool configured[64] = {false};
   int dev = 0;
   const int sms = device_sms(&dev);
@@ -443,7 +581,7 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const GemmArgs &g,
   }
   const int units = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN) * g.splits;
   const int grid = units < sms ? units : sms;
-  kern<<<grid, NTHREADS, smem, st>>>(ma, mb, g);
+  kern<<<grid, NTHREADS, smem, st>>>(ma, mb, mo, mo2, g);
   return sv::after_launch();
 }
 
@@ -477,10 +615,16 @@ int pick_tile(int M, int N, int sms, bool wgrad) {
 }
 
 template <int EPI, int TA, int TB>
-int dispatch(int bn, const CUtensorMap &ma, const CUtensorMap &mb, const GemmArgs &g, cudaStream_t st) {
-  if (bn == 192) return launch_gemm<192, EPI, TA, TB>(ma, mb, g, st);
-  if (bn == 128) return launch_gemm<128, EPI, TA, TB>(ma, mb, g, st);
-  return launch_gemm<64, EPI, TA, TB>(ma, mb, g, st);
+int dispatch(int bn, bool tma, const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mo, const CUtensorMap &mo2,
+             const GemmArgs &g, cudaStream_t st) {
+  if (tma) {
+    if (bn == 192) return launch_gemm<192, EPI, TA, TB, 1>(ma, mb, mo, mo2, g, st);
+    if (bn == 128) return launch_gemm<128, EPI, TA, TB, 1>(ma, mb, mo, mo2, g, st);
+    return launch_gemm<64, EPI, TA, TB, 1>(ma, mb, mo, mo2, g, st);
+  }
+  if (bn == 192) return launch_gemm<192, EPI, TA, TB, 0>(ma, mb, mo, mo2, g, st);
+  if (bn == 128) return launch_gemm<128, EPI, TA, TB, 0>(ma, mb, mo, mo2, g, st);
+  return launch_gemm<64, EPI, TA, TB, 0>(ma, mb, mo, mo2, g, st);
 }
 
 int g_force_bn = 0;     // tests / benchmarks: 1, 2 or 4 forces 64-, 128- or 192-column tiles, 0 = heuristic
@@ -525,12 +669,32 @@ int run_gemm(int epi, const void *A, int lda, int a_t, const void *B, int ldb, i
   if (rc) return rc;
   rc = b_t ? make_map_mn(&mb, B, N, K, ldb) : make_map(&mb, B, N, K, ldb, bn);
   if (rc) return rc;
-  if (epi == EPI_FWD) {
-    if (a_t) return b_t ? dispatch<EPI_FWD, 1, 1>(bn, ma, mb, g, st) : dispatch<EPI_FWD, 1, 0>(bn, ma, mb, g, st);
-    return b_t ? dispatch<EPI_FWD, 0, 1>(bn, ma, mb, g, st) : dispatch<EPI_FWD, 0, 0>(bn, ma, mb, g, st);
+  // The epilogue goes out through shared memory by TMA whenever the output rows can take 16-byte-aligned boxes.  The output
+  // maps span only the columns that fill whole 16-byte units (n_tma); the last few columns of a width like 607 or 30522 are
+  // stored per element by the epilogue itself.  A TMA store clips a box at the map's inner dim only to 16-byte granularity
+  // (on H100, N = 607 in bf16 wrote column 607), so a map of width N would write into the pad columns.  The SA3 row max, the
+  // residual add and odd pitches keep the per-element stores.
+  const int esz = epi == EPI_WGRAD || g.out_f32 ? 4 : 2;
+  g.n_tma = (int)(((size_t)N * esz / 16) * 16 / esz);
+  auto al16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  const bool tma = g.rowmax == 0 && g.residual == nullptr && g.ldo >= N && ((size_t)g.ldo * esz) % 16 == 0 && g.n_tma > 0 &&
+                   al16(g.out) && (g.out2 == nullptr || (esz == 2 && al16(g.out2)));
+  CUtensorMap mo{}, mo2{};
+  if (tma) {
+    rc = make_out_map(&mo, g.out, M, g.n_tma, g.ldo, esz == 4);
+    if (rc) return rc;
+    if (g.out2 != nullptr) {
+      rc = make_out_map(&mo2, g.out2, M, g.n_tma, g.ldo, false);
+      if (rc) return rc;
+    }
   }
-  if (epi == EPI_DGRAD && !a_t && b_t) return dispatch<EPI_DGRAD, 0, 1>(bn, ma, mb, g, st);
-  if (epi == EPI_WGRAD && a_t && b_t) return dispatch<EPI_WGRAD, 1, 1>(bn, ma, mb, g, st);
+  if (epi == EPI_FWD) {
+    if (a_t)
+      return b_t ? dispatch<EPI_FWD, 1, 1>(bn, tma, ma, mb, mo, mo2, g, st) : dispatch<EPI_FWD, 1, 0>(bn, tma, ma, mb, mo, mo2, g, st);
+    return b_t ? dispatch<EPI_FWD, 0, 1>(bn, tma, ma, mb, mo, mo2, g, st) : dispatch<EPI_FWD, 0, 0>(bn, tma, ma, mb, mo, mo2, g, st);
+  }
+  if (epi == EPI_DGRAD && !a_t && b_t) return dispatch<EPI_DGRAD, 0, 1>(bn, tma, ma, mb, mo, mo2, g, st);
+  if (epi == EPI_WGRAD && a_t && b_t) return dispatch<EPI_WGRAD, 1, 1>(bn, tma, ma, mb, mo, mo2, g, st);
   return SV_ERR_INVALID_ARG;
 }
 

@@ -52,6 +52,34 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const void *map, 
       : "memory");
 }
 
+// ---- TMA: one 2-D box shared -> global, as a store or an fp32/bf16 reduce-add; tracked by the issuing thread's bulk groups.
+// The box must have been written through the generic proxy before a fence_proxy_async_smem().  Elements outside the
+// tensor map's global dims are not written.
+__device__ __forceinline__ void tma_store_2d(const void *map, uint32_t src_smem, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src_smem), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_reduce_add_2d(const void *map, uint32_t src_smem, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src_smem), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every committed bulk group of this thread has completed (its global writes included)
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// four 8x8 b16 matrices -> shared: lane l gives the address of row l % 8 of matrix l / 8; register q holds this lane's
+// two elements (row l / 4, columns 2 (l % 4) + {0, 1}) of matrix q — the layout of a wgmma accumulator's 8x8 blocks
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+
 // ---- wgmma descriptors ----------------------------------------------------------------------------
 // shared-memory matrix descriptor, SWIZZLE_128B (layout type 1 in bits [62,64)): [0,14) start >> 4 | [16,30) leading
 // byte offset >> 4 | [32,46) stride byte offset >> 4.  The stride byte offset is the distance between 8-row (K-major) or
