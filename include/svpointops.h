@@ -103,6 +103,67 @@ int sv_sa_sample_f32(const float *xyz, int B, int N, int m, float radius, int ns
  * NULL (receives the chosen raw indices, -1 for empty slots).  Randomness = counter hash of (seed, slot, k). */
 int sv_scene_prep_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int P, unsigned long long seed,
                       float *obj_fts, float *obj_locs, unsigned char *obj_masks, int *sample_idx, void *stream);
+/* Training-split object augmentation (the `data_aug` configs): restates data/datasets/data_augmentor.py
+ * `DataAugmentor.update_data_dict` followed by data/datasets/base.py:742-776 `_obj_processing_aug`, per object slot, in this
+ * order: scene flip of all raw xyz; scene scaling about the raw mean (taken after the flip); subsample P points (without
+ * replacement when n >= P); jitter x + (g - 0.5) * jitter; size = max - min HERE (after the jitter, before translation and
+ * rotation, so a 90 degree scene rotation does not swap the sizes); + scene translation, + object translation; x @ R_scene;
+ * object rotation (x - c) @ R_obj + c about the mean of the P points; + rgb_delta on the colours; point shuffle.  Outputs:
+ * obj_locs = [mean xyz, size], obj_boxes = [(min + max) / 2, size], obj_fts xyz = (x - mean) / max(max norm, 1e-6).
+ * Padded slots (empty range): all-ones points, zero locs / boxes, mask 0.
+ *
+ * Which transforms run is `params->flags` (SV_AUG_*); their random values come from two tables:
+ *   item_tab (n_items, SV_AUG_ITEM_STRIDE) f64 = [flip 3x3 | scale | scene translation 3 | scene rotation 3x3 | rgb delta 3]
+ *   obj_tab  (n_items * slots_per_item, SV_AUG_OBJ_STRIDE) f64 = [object translation 3 | object rotation 3x3]
+ * (matrices row-major, applied as x @ M like the reference).  sv_aug_draw fills them from a seed; a caller may fill them itself
+ * (replaying recorded draws).  Per output point: index_in (n_slots, P) i32 = the raw index of output position k (subsample
+ * composed with the shuffle) and noise_in (n_slots, P, 3) f32 = the standard normals of its jitter.  Either may be NULL: it is
+ * then drawn from (seed, slot, k); noise_in is read only with SV_AUG_JITTER.  index_out / noise_out (same layouts, NULL-able)
+ * receive what was used (-1 / 0 on padded slots), so feeding them back as index_in / noise_in with the same tables reproduces
+ * the output bit for bit.  obj_boxes (n_slots, 6) may be NULL.  All raw points are read only with SV_AUG_SCALE (the raw mean);
+ * otherwise just the P gathered rows.  1 <= P <= 8192. */
+#define SV_AUG_FLIP 1
+#define SV_AUG_SCALE 2
+#define SV_AUG_SCENE_TRANS 4
+#define SV_AUG_SCENE_ROT 8
+#define SV_AUG_COLOR 16
+#define SV_AUG_OBJ_TRANS 32
+#define SV_AUG_OBJ_ROT 64
+#define SV_AUG_JITTER 128
+#define SV_AUG_PTS_SHUFFLE 256
+#define SV_AUG_ITEM_STRIDE 25
+#define SV_AUG_OBJ_STRIDE 12
+typedef struct {
+  int flags;                       /* SV_AUG_* */
+  int scene_rot_axis_align, scene_rot_shuffle, obj_rot_axis_align, obj_rot_shuffle;
+  double scale_lo, scale_hi;       /* scene scaling s ~ U[lo, hi] */
+  double scene_trans[3];           /* scene translation N(0,1) * value[i] */
+  double scene_rot[3];             /* rotation value[i] (scales each angle) */
+  double obj_trans[3];
+  double obj_rot[3];
+  double jitter;                   /* random_jitter value */
+} sv_aug_params;
+/* Fills item_tab / obj_tab (layouts above) from (seed, item / slot): flip type uniform over {x, y, x and y, none}; s = U * (hi -
+ * lo) + lo; translations N(0,1) * value; rotations built as data_augmentor.py builds rx, ry, rz (angle = choice of {0, pi/2, pi,
+ * 3 pi/2} * value with axis_align, else (U * 2 pi - pi) * value), multiplied in a uniformly random order with shuffle; rgb delta
+ * N(0,1) * 0.1.  Entries of disabled transforms are identity / zero. */
+int sv_aug_draw(const sv_aug_params *params, int n_items, int slots_per_item, unsigned long long seed, double *item_tab,
+                double *obj_tab, void *stream);
+int sv_scene_prep_aug_f32(const float *raw_points, const long long *slot_offsets, int n_items, int slots_per_item, int P,
+                          const sv_aug_params *params, const double *item_tab, const double *obj_tab, const int *index_in,
+                          const float *noise_in, unsigned long long seed, float *obj_fts, float *obj_locs, float *obj_boxes,
+                          unsigned char *obj_masks, int *index_out, float *noise_out, void *stream);
+/* `_obj_processing_post` with `rot_aug` (data/datasets/base.py:697-741, data/data_utils.py:163-178 `build_rotate_mat`): the
+ * raw xyz of every object of item b are first rotated x @ R^T, R = [[c, -s, 0], [s, c, 0], [0, 0, 1]] in f32 with theta =
+ * quarter_turns[b] * pi / 2 (0 = not rotated), then processed exactly as sv_scene_prep_f32 does.  quarter_turns (n_slots /
+ * slots_per_item) i32 in 0..3 may be NULL (no rotation: then obj_fts / obj_locs / obj_masks / sample_idx equal
+ * sv_scene_prep_f32's for the same seed).  obj_boxes (n_slots, 6) = [(min + max) / 2, max - min] of the rotated raw points, may
+ * be NULL.  index_in (n_slots, P) i32 may be NULL (drawn from the seed as in sv_scene_prep_f32) or give the sampled raw indices.
+ * sv_quarter_turn_draw fills quarter_turns (n_items) uniformly from the seed. */
+int sv_scene_prep_rot_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int slots_per_item, int P,
+                          unsigned long long seed, const int *quarter_turns, const int *index_in, float *obj_fts,
+                          float *obj_locs, float *obj_boxes, unsigned char *obj_masks, int *sample_idx, void *stream);
+int sv_quarter_turn_draw(int n_items, unsigned long long seed, int *quarter_turns, void *stream);
 /* BERT masked-LM corruption (data/data_utils.py:76-104 `random_word`): for tokens with attention_mask != 0, with probability
  * mask_ratio the label is the original id and the token becomes [MASK] (80 %), a uniform random id (10 %) or stays (10 %);
  * every other label is -1.  ids / attention_mask / out_ids / labels: (n_tokens) int64. */

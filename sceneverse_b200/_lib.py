@@ -8,6 +8,20 @@ _cache = {}
 
 c_int, c_float, c_void_p = ctypes.c_int, ctypes.c_float, ctypes.c_void_p
 
+# include/svpointops.h sv_aug_params
+AUG_FLIP, AUG_SCALE, AUG_SCENE_TRANS, AUG_SCENE_ROT, AUG_COLOR = 1, 2, 4, 8, 16
+AUG_OBJ_TRANS, AUG_OBJ_ROT, AUG_JITTER, AUG_PTS_SHUFFLE = 32, 64, 128, 256
+AUG_ITEM_STRIDE, AUG_OBJ_STRIDE = 25, 12
+
+
+class AugParams(ctypes.Structure):
+    _fields_ = [("flags", c_int), ("scene_rot_axis_align", c_int), ("scene_rot_shuffle", c_int),
+                ("obj_rot_axis_align", c_int), ("obj_rot_shuffle", c_int),
+                ("scale_lo", ctypes.c_double), ("scale_hi", ctypes.c_double),
+                ("scene_trans", ctypes.c_double * 3), ("scene_rot", ctypes.c_double * 3),
+                ("obj_trans", ctypes.c_double * 3), ("obj_rot", ctypes.c_double * 3), ("jitter", ctypes.c_double)]
+
+
 _POINTOPS_SIGS = {
     # name: argtypes
     "sv_fps_f32": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
@@ -21,6 +35,13 @@ _POINTOPS_SIGS = {
     "sv_three_interpolate_grad_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
     "sv_fps_ballquery_f32": [c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
     "sv_scene_prep_f32": [c_void_p, c_void_p, c_int, c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sv_scene_prep_rot_f32": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sv_quarter_turn_draw": [c_int, ctypes.c_ulonglong, c_void_p, c_void_p],
+    "sv_aug_draw": [ctypes.POINTER(AugParams), c_int, c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p],
+    "sv_scene_prep_aug_f32": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(AugParams), c_void_p, c_void_p, c_void_p,
+                              c_void_p, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                              c_void_p],
     "sv_token_mask": [c_void_p, c_void_p, ctypes.c_longlong, c_float, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_ulonglong,
                       c_void_p, c_void_p, c_void_p],
     "sv_coin_mask": [c_void_p, ctypes.c_longlong, c_float, ctypes.c_ulonglong, c_void_p, c_void_p],

@@ -5,7 +5,16 @@ data/datasets/dataset_wrapper.py:38-111 (padding, masks) and data/data_utils.py:
 Input (what a scan loader hands over after reading the files): every object's raw points concatenated (total, 6) [xyz rgb],
 a CSR offset per object SLOT (B * max_obj_len + 1; padded slots are empty ranges), the tokenised captions.  Output: the keys
 `OpenVocab.forward` consumes, same dtypes and padding conventions as the reference (padded objects = all-ones points, zero
-locs, label -100, mask False).  Randomness is a counter hash of (seed, index): reproducible and order independent."""
+locs, label -100, mask False).  Randomness is a counter hash of (seed, index): reproducible and order independent.
+
+The training split of a config is augmented as the reference's dataset does it (`AugSpec`, `prepare_objects_aug`): with a
+`data_aug` block, data/datasets/data_augmentor.py + base.py:742-776 `_obj_processing_aug`; without one, `_obj_processing_post`
+with its `rot_aug` quarter turn (data/data_utils.py:163-178)."""
+import math
+from collections.abc import Mapping
+from dataclasses import dataclass
+from typing import Optional, Tuple
+
 import torch
 
 from . import _lib
@@ -36,6 +45,241 @@ def prepare_objects(raw_points, slot_offsets, B, O, P=1024, seed=0, return_indic
     return out + (idx,) if return_indices else out
 
 
+@dataclass(frozen=True)
+class RotationSpec:
+    """One `rotation` block of data_augmentor.py: angle i is value[i] times a quarter turn (axis_align) or U[-pi, pi)."""
+    value: Tuple[float, float, float]
+    axis_align: bool
+    shuffle: bool
+
+
+@dataclass(frozen=True)
+class AugSpec:
+    """Which object-processing path runs and which augmentations it applies.
+
+    path "aug": the config has a `data_aug` block (base.py:247-253, 964-972), every field below may be set.
+    path "post": no `data_aug`; only `rot_aug` (a quarter turn per item, train split) applies."""
+    path: str = "post"
+    rot_aug: bool = False
+    flip: bool = False
+    scaling: Optional[Tuple[float, float]] = None
+    scene_translation: Optional[Tuple[float, float, float]] = None
+    scene_rotation: Optional[RotationSpec] = None
+    color_jitter: bool = False
+    obj_translation: Optional[Tuple[float, float, float]] = None
+    obj_rotation: Optional[RotationSpec] = None
+    jitter: Optional[float] = None
+    pts_shuffle: bool = False
+
+    @classmethod
+    def from_config(cls, data_aug, rot_aug=False, split="train"):
+        """Restates how the reference picks the path and builds `DataAugmentor`'s queue.  `data_aug` may be a plain mapping or
+        an attribute-style config (hydra's DictConfig).  An augmentation runs only on the train split, when it is named in
+        `aug_list` and present in the block, and when `check_key` enables it (None / bool / `enabled`; a missing entry counts
+        as absent).  `p` is not consulted: the reference's blocks are DictConfigs, not dicts, so its `check_p` is always true.
+        `order_shuffle` (a permutation nothing reads) and `accord_to_size` (never read) are accepted and ignored."""
+        if not data_aug:
+            return cls(path="post", rot_aug=bool(rot_aug) and split == "train")
+        if split != "train":
+            return cls(path="aug")
+        aug_list = _cfg_get(data_aug, "aug_list")
+        if aug_list is None or isinstance(aug_list, (str, bytes)):
+            raise ValueError(f"data_aug.aug_list must be a list of augmentation names, got {aug_list!r}")
+        kw = {}
+        for aug in aug_list:
+            if not _cfg_has(data_aug, aug):
+                continue
+            block = _cfg_get(data_aug, aug)
+            if aug == "scene_aug":
+                if _check_key(_cfg_get(block, "translation")):
+                    kw["scene_translation"] = _vec3(_cfg_get(_cfg_get(block, "translation"), "value"), "scene_aug.translation.value")
+                if _check_key(_cfg_get(block, "scaling")):
+                    kw["scaling"] = _pair(_cfg_get(_cfg_get(block, "scaling"), "value"), "scene_aug.scaling.value")
+                kw["flip"] = bool(_check_key(_cfg_get(block, "flip")))
+                if _check_key(_cfg_get(block, "rotation")):
+                    kw["scene_rotation"] = _rotation(_cfg_get(block, "rotation"), "scene_aug.rotation")
+                kw["color_jitter"] = bool(_check_key(_cfg_get(block, "color_jitter")))
+            elif aug == "obj_aug":
+                if _check_key(_cfg_get(block, "translation")):
+                    kw["obj_translation"] = _vec3(_cfg_get(_cfg_get(block, "translation"), "value"), "obj_aug.translation.value")
+                if _check_key(_cfg_get(block, "rotation")):
+                    kw["obj_rotation"] = _rotation(_cfg_get(block, "rotation"), "obj_aug.rotation")
+                if _check_key(_cfg_get(block, "random_jitter")):
+                    v = _number(_cfg_get(_cfg_get(block, "random_jitter"), "value"), "obj_aug.random_jitter.value")
+                    if v < 0:
+                        raise ValueError(f"obj_aug.random_jitter.value must be >= 0, got {v}")
+                    kw["jitter"] = v
+                kw["pts_shuffle"] = bool(_check_key(_cfg_get(block, "pts_shuffle")))
+            else:
+                raise ValueError(f"unknown augmentation {aug!r} in data_aug.aug_list (known: scene_aug, obj_aug)")
+        return cls(path="aug", **kw)
+
+    def params(self):
+        """The C-side `sv_aug_params` of the aug path."""
+        p = _lib.AugParams()
+        f = 0
+        if self.flip:
+            f |= _lib.AUG_FLIP
+        if self.scaling is not None:
+            f |= _lib.AUG_SCALE
+            p.scale_lo, p.scale_hi = self.scaling
+        if self.scene_translation is not None:
+            f |= _lib.AUG_SCENE_TRANS
+            p.scene_trans[:] = self.scene_translation
+        if self.scene_rotation is not None:
+            f |= _lib.AUG_SCENE_ROT
+            p.scene_rot[:] = self.scene_rotation.value
+            p.scene_rot_axis_align, p.scene_rot_shuffle = int(self.scene_rotation.axis_align), int(self.scene_rotation.shuffle)
+        if self.color_jitter:
+            f |= _lib.AUG_COLOR
+        if self.obj_translation is not None:
+            f |= _lib.AUG_OBJ_TRANS
+            p.obj_trans[:] = self.obj_translation
+        if self.obj_rotation is not None:
+            f |= _lib.AUG_OBJ_ROT
+            p.obj_rot[:] = self.obj_rotation.value
+            p.obj_rot_axis_align, p.obj_rot_shuffle = int(self.obj_rotation.axis_align), int(self.obj_rotation.shuffle)
+        if self.jitter is not None:
+            f |= _lib.AUG_JITTER
+            p.jitter = self.jitter
+        if self.pts_shuffle:
+            f |= _lib.AUG_PTS_SHUFFLE
+        p.flags = f
+        return p
+
+
+def _cfg_has(cfg, key):
+    if cfg is None or isinstance(cfg, (bool, int, float, str)):
+        return False
+    if isinstance(cfg, Mapping) or hasattr(cfg, "keys"):
+        return key in cfg
+    return hasattr(cfg, key)
+
+
+def _cfg_get(cfg, key, default=None):
+    if not _cfg_has(cfg, key):
+        return default
+    if isinstance(cfg, Mapping) or hasattr(cfg, "keys"):
+        return cfg[key]
+    return getattr(cfg, key)
+
+
+def _check_key(key):
+    """data_augmentor.py DataAugmentor.check_key."""
+    if key is None:
+        return False
+    if isinstance(key, bool):
+        return key
+    if isinstance(key, dict):
+        return key.get("enabled", True)
+    if _cfg_has(key, "enabled"):
+        return _cfg_get(key, "enabled")
+    return True
+
+
+def _number(v, what):
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+        raise ValueError(f"{what} must be a finite number, got {v!r}")
+    return float(v)
+
+
+def _seq(v, n, what):
+    if v is None or isinstance(v, (str, bytes, Mapping)) or not hasattr(v, "__len__") or len(v) != n:
+        raise ValueError(f"{what} must be a list of {n} numbers, got {v!r}")
+    return tuple(_number(x, what) for x in v)
+
+
+def _vec3(v, what):
+    return _seq(v, 3, what)
+
+
+def _pair(v, what):
+    return _seq(v, 2, what)
+
+
+def _rotation(block, what):
+    return RotationSpec(_vec3(_cfg_get(block, "value"), what + ".value"), bool(_cfg_get(block, "axis_align", False)),
+                        bool(_cfg_get(block, "shuffle", False)))
+
+
+def prepare_objects_aug(raw_points, slot_offsets, B, O, P, spec, seed, want_boxes=False, draws=None, return_draws=False):
+    """The object tensors of one batch with the augmentation `spec` (AugSpec) of a training split.
+
+    raw_points (total,6) f32 cuda, slot_offsets (B*O+1) int64 cuda (O slots per item, empty range = padded slot) ->
+    obj_fts (B,O,P,6) f32, obj_locs (B,O,6) f32, obj_masks (B,O) bool [, obj_boxes (B,O,6) f32 if want_boxes]
+    [, draws if return_draws].
+
+    The random values come from `seed`, or from `draws` (replay):
+      aug path:  {"item": (B,25) f64, "obj": (B,O,12) f64, "index": (B,O,P) i32, "noise": (B,O,P,3) f32 (with jitter)}
+                 (table layouts in include/svpointops.h; index = the raw index of each output point, subsample and shuffle
+                 composed; noise = the standard normals of its jitter);
+      post path: {"quarter_turns": (B,) i32 in 0..3, "index": (B,O,P) i32}.
+    `return_draws` returns the dict that was used; passing it back as `draws` reproduces the output bit for bit."""
+    assert raw_points.is_cuda and raw_points.dtype == torch.float32 and raw_points.dim() == 2 and raw_points.shape[1] == 6
+    assert slot_offsets.dtype == torch.int64 and slot_offsets.numel() == B * O + 1
+    if spec.path not in ("aug", "post"):
+        raise ValueError(f"unknown object-processing path {spec.path!r}")
+    raw_points, slot_offsets = raw_points.contiguous(), slot_offsets.contiguous()
+    dev = raw_points.device
+    fts = torch.empty((B, O, P, 6), dtype=torch.float32, device=dev)
+    locs = torch.empty((B, O, 6), dtype=torch.float32, device=dev)
+    masks = torch.empty((B, O), dtype=torch.uint8, device=dev)
+    boxes = torch.empty((B, O, 6), dtype=torch.float32, device=dev) if want_boxes else None
+    seed = int(seed) & 0x7FFFFFFFFFFFFFFF
+    lib = _lib.pointops()
+
+    def ptr(t):
+        return t.data_ptr() if t is not None else None
+
+    def given(key, shape, dtype):
+        t = draws.get(key)
+        if t is None or tuple(t.shape) != shape or t.dtype != dtype or t.device != dev:
+            raise ValueError(f"draws[{key!r}] must be a {dtype} tensor of shape {shape} on {dev}")
+        return t.contiguous()
+
+    st = _stream(raw_points)
+    with torch.cuda.device(dev):
+        if spec.path == "post":
+            if draws is not None:
+                qt, idx_in = given("quarter_turns", (B,), torch.int32), given("index", (B, O, P), torch.int32)
+            else:
+                qt, idx_in = None, None
+                if spec.rot_aug:
+                    qt = torch.empty(B, dtype=torch.int32, device=dev)
+                    _lib.check(lib, lib.sv_quarter_turn_draw(B, seed, qt.data_ptr(), st), "sv_quarter_turn_draw")
+            idx_out = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_draws else None
+            rc = lib.sv_scene_prep_rot_f32(raw_points.data_ptr(), slot_offsets.data_ptr(), B * O, O, P, seed, ptr(qt), ptr(idx_in),
+                                           fts.data_ptr(), locs.data_ptr(), ptr(boxes), masks.data_ptr(), ptr(idx_out), st)
+            _lib.check(lib, rc, "sv_scene_prep_rot_f32")
+            used = {"quarter_turns": qt if qt is not None else torch.zeros(B, dtype=torch.int32, device=dev),
+                    "index": idx_out}
+        else:
+            params = spec.params()
+            jitter = spec.jitter is not None
+            if draws is not None:
+                item, obj = given("item", (B, _lib.AUG_ITEM_STRIDE), torch.float64), given("obj", (B, O, _lib.AUG_OBJ_STRIDE), torch.float64)
+                idx_in = given("index", (B, O, P), torch.int32)
+                noise_in = given("noise", (B, O, P, 3), torch.float32) if jitter else None
+            else:
+                item = torch.empty((B, _lib.AUG_ITEM_STRIDE), dtype=torch.float64, device=dev)
+                obj = torch.empty((B, O, _lib.AUG_OBJ_STRIDE), dtype=torch.float64, device=dev)
+                idx_in = noise_in = None
+                _lib.check(lib, lib.sv_aug_draw(params, B, O, seed, item.data_ptr(), obj.data_ptr(), st), "sv_aug_draw")
+            idx_out = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_draws else None
+            noise_out = torch.empty((B, O, P, 3), dtype=torch.float32, device=dev) if return_draws and jitter else None
+            rc = lib.sv_scene_prep_aug_f32(raw_points.data_ptr(), slot_offsets.data_ptr(), B, O, P, params, item.data_ptr(),
+                                           obj.data_ptr(), ptr(idx_in), ptr(noise_in), seed, fts.data_ptr(), locs.data_ptr(),
+                                           ptr(boxes), masks.data_ptr(), ptr(idx_out), ptr(noise_out), st)
+            _lib.check(lib, rc, "sv_scene_prep_aug_f32")
+            used = {"item": item, "obj": obj, "index": idx_out}
+            if jitter:
+                used["noise"] = noise_out
+    out = (fts, locs, masks.bool())
+    if want_boxes:
+        out += (boxes,)
+    return out + (used,) if return_draws else out
+
+
 def mask_tokens(txt_ids, txt_masks, mask_ratio=0.15, mask_token_id=103, vocab_size=30522, seed=0):
     """BERT masked-LM corruption: (B,L) int64 ids / masks -> (masked ids, labels with -1 = not supervised)."""
     assert txt_ids.is_cuda and txt_ids.dtype == torch.int64 and txt_masks.dtype == torch.int64 and txt_ids.shape == txt_masks.shape
@@ -61,13 +305,23 @@ def mask_objects(obj_masks, drop_ratio=0.1, seed=0):
 
 
 def build_data_dict(raw_points, slot_offsets, obj_labels, txt_ids, txt_masks, tgt_object_id, B, O, P=1024, seed=0,
-                    txt_mask_ratio=0.15, pc_mask_ratio=0.1, scene_txt_ids=None, scene_txt_masks=None):
+                    txt_mask_ratio=0.15, pc_mask_ratio=0.1, scene_txt_ids=None, scene_txt_masks=None, augment=None,
+                    want_boxes=False):
     """Everything `OpenVocab.forward` + the losses read, in three launches.  obj_labels: (B,O) int64 with -100 on padded slots
-    (dataset_wrapper.py:70-71); tgt_object_id (B,1) int64."""
-    fts, locs, masks = prepare_objects(raw_points, slot_offsets, B, O, P, seed)
+    (dataset_wrapper.py:70-71); tgt_object_id (B,1) int64.  augment: an AugSpec (`AugSpec.from_config(cfg.data_aug,
+    cfg.data.args.rot_aug, split)`) processes the objects as that config's split does; None keeps the plain post path of
+    `prepare_objects`.  want_boxes adds "obj_boxes" (B,O,6) = [box centre, size]."""
+    if augment is None and not want_boxes:
+        fts, locs, masks = prepare_objects(raw_points, slot_offsets, B, O, P, seed)
+    else:
+        objs = prepare_objects_aug(raw_points, slot_offsets, B, O, P, augment if augment is not None else AugSpec(), seed,
+                                   want_boxes=want_boxes)
+        fts, locs, masks = objs[:3]
     ids, labels = mask_tokens(txt_ids, txt_masks, txt_mask_ratio, seed=seed + 1)
     d = {"obj_fts": fts, "obj_locs": locs, "obj_masks": masks, "obj_sem_masks": mask_objects(masks, pc_mask_ratio, seed + 2),
          "obj_labels": obj_labels, "txt_ids": ids, "txt_masks": txt_masks, "masked_lm_labels": labels, "tgt_object_id": tgt_object_id}
+    if want_boxes:
+        d["obj_boxes"] = objs[3]
     if scene_txt_ids is not None:
         d["scene_txt_ids"], d["scene_txt_masks"] = scene_txt_ids, scene_txt_masks
     return d
