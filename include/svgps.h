@@ -311,6 +311,53 @@ int sv_normalize_allgather_dev_f32(const float *a, const float *b, int n, int D,
                                    void *const *peer_signals, unsigned *done_counter, int world, int rank,
                                    unsigned *epoch_dev, void *stream);
 
+/* Evaluation metrics (csrc/eval_metrics.cu; reference: evaluator/*.py `batch_metrics`).  Each evaluator owns one zeroed device
+ * vector of sv_eval_counters_size(kind) doubles; the kernels ADD one batch into it (atomics, CUDA-graph replay safe).  Counts
+ * are integers held exactly in float64.  Logits are bf16 (is_bf16 != 0) or f32 rows with a row stride in elements (padded
+ * vocabularies are read in place).  valid: (B,) bytes or NULL (all valid); an item with valid 0 counts nothing. */
+enum { SV_EVAL_GROUNDING = 0, SV_EVAL_OBJ_CLS = 1, SV_EVAL_ANSWERS = 2 };
+/* ScanReferEval / ReferIt3DEval: items; is_multiple / is_hard / is_view_dependent items; og_pred == tgt_object_id (all, hard,
+ * view-dependent); IoU-25 / IoU-50 flag at og_pred (all, multiple); txt_acc; then up to three (hits, masked objects) pairs of
+ * sv_eval_obj_cls at SV_EVG_OBJ. */
+enum {
+  SV_EVG_ITEMS = 0, SV_EVG_MULTIPLE, SV_EVG_HARD, SV_EVG_VIEW_DEP, SV_EVG_OG_ACC, SV_EVG_OG_ACC_HARD, SV_EVG_OG_ACC_VIEW_DEP,
+  SV_EVG_IOU25, SV_EVG_IOU50, SV_EVG_IOU25_MULTIPLE, SV_EVG_IOU50_MULTIPLE, SV_EVG_TXT_ACC, SV_EVG_OBJ, SV_EVG_SIZE = SV_EVG_OBJ + 6
+};
+/* PretrainObjEval: one (hits, masked objects) pair */
+enum { SV_EVO_HIT = 0, SV_EVO_COUNT = 1, SV_EVO_SIZE = 2 };
+/* ScanQAEval / SQA3DEval: items, top-1 and top-10 hits, items and top-1 hits per sqa_type (6 types), the (hits, masked
+ * objects) pair of obj_cls_raw; then SQA3DEval's state: a snapshot of those integers at the end of the previous batch and its
+ * float64 sums of per-batch ratio x batch size (ans1 = target_metric, ans10, obj_cls_raw, type k) and of the type counts. */
+enum {
+  SV_EVA_NTYPES = 6,
+  SV_EVA_ITEMS = 0, SV_EVA_ANS1 = 1, SV_EVA_ANS10 = 2, SV_EVA_TYPE_ITEMS = 3, SV_EVA_TYPE_ANS1 = 9, SV_EVA_OBJ_HIT = 15,
+  SV_EVA_OBJ_COUNT = 16, SV_EVA_SNAPSHOT = 17, SV_EVA_Q_ANS1 = 34, SV_EVA_Q_ANS10 = 35, SV_EVA_Q_OBJ = 36, SV_EVA_Q_TYPE = 37,
+  SV_EVA_Q_TYPE_COUNT = 43, SV_EVA_SIZE = 49
+};
+int sv_eval_counters_size(int kind);
+/* og_pred = argmax of og3d_logits (B, O) (torch's rule: first maximum, NaN above everything), element (b, o) at
+ * b * og_row_stride + o * og_col_stride (the grounding head writes it as column 0 of padded rows).  tgt_object_id (B) int64.
+ * iou25 / iou50: (B, >= O) int64 rows or both NULL (ReferIt3D).  txt_cls_logits (B, txt_classes) rows or NULL, against
+ * tgt_object_label (B) int64.  Flags: (B) bytes or NULL (= 0). */
+int sv_eval_grounding(const void *og3d_logits, int og_bf16, long long og_row_stride, long long og_col_stride, int B, int O,
+                      const long long *tgt_object_id, const long long *iou25, const long long *iou50, long long iou_row_stride,
+                      const void *txt_cls_logits, int txt_bf16, long long txt_row_stride, int txt_classes,
+                      const long long *tgt_object_label, const unsigned char *is_multiple, const unsigned char *is_hard,
+                      const unsigned char *is_view_dependent, const unsigned char *valid, double *counters, void *stream);
+/* Up to three (B, O, C) logits tensors (host arrays of device pointers / dtypes / strides in elements): for tensor t,
+ * counters[2t] += #{masked objects whose argmax over C equals obj_labels}, counters[2t + 1] += #{masked objects}.
+ * obj_labels (B, O) int64, obj_masks (B, O) bytes. */
+int sv_eval_obj_cls(int n_logits, const void *const *logits, const int *is_bf16, const long long *row_stride,
+                    const long long *item_stride, int B, int O, int C, const long long *obj_labels,
+                    const unsigned char *obj_masks, const unsigned char *valid, double *counters, void *stream);
+/* answer_scores (B, A) rows; answer_label (B, A) int64 multi-hot (a 1 marks a correct answer).  Top-1 hit: the argmax is
+ * labelled 1.  Top-10 hit: a labelled answer ranks among the first 10 (scores descending, NaN first, ties: lower index first).
+ * sqa_type (B) int64 in 0..5 or NULL.  Adds into the SV_EVA_* words. */
+int sv_eval_answers(const void *answer_scores, int is_bf16, long long row_stride, int B, int A, const long long *answer_label,
+                    const long long *sqa_type, const unsigned char *valid, double *counters, void *stream);
+/* SQA3DEval.update's float64 bookkeeping for the batch just added (after sv_eval_answers and sv_eval_obj_cls of that batch). */
+int sv_eval_sqa3d_batch(double *counters, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

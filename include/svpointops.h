@@ -174,6 +174,20 @@ int sv_token_mask(const long long *ids, const long long *attention_mask, long lo
 int sv_coin_mask(const unsigned char *valid, long long n, float drop_ratio, unsigned long long seed, unsigned char *out,
                  void *stream);
 
+/* Evaluation targets of the grounding datasets (csrc/eval_targets.cu; reference: data/datasets/base.py:387-454), one CTA per
+ * item.  points (total, 6) f32 [xyz rgb]; cand_offsets: CSR over points, one range per candidate object (each >= 1 point);
+ * item_offsets (B + 1): the candidates of item b are cand_offsets ranges item_offsets[b] .. item_offsets[b+1]-1, at most
+ * max_cand (<= 4096) of them.  pred mode (gt_index NULL): gt_points / gt_offsets (B + 1) hold each item's ground-truth object;
+ * IoU of the numpy-1.26 box round trip, hits at >= 0.25 / >= 0.5, target = the last IoU-25 hit.  gt mode: gt_index (B) int64
+ * is the target candidate (local index) and its only hit.  cand_labels (n_cand) int64, tgt_label (B) int64.
+ * Outputs: slot_map (B, O) int32 = local candidate index per slot in ascending order, -1 = empty; tgt_object_id (B) int64 = the
+ * target's slot or the kept count when there is none; iou25 / iou50 (B, O) int64 flags per slot; iou_out (n_cand) f32 or NULL. */
+int sv_grounding_targets_f32(const float *points, const long long *cand_offsets, const long long *item_offsets,
+                             const float *gt_points, const long long *gt_offsets, const long long *gt_index,
+                             const long long *cand_labels, const long long *tgt_label, int B, int O, int max_cand,
+                             unsigned long long seed, int *slot_map, long long *tgt_object_id, long long *iou25,
+                             long long *iou50, float *iou_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

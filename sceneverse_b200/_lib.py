@@ -14,6 +14,17 @@ AUG_OBJ_TRANS, AUG_OBJ_ROT, AUG_JITTER, AUG_PTS_SHUFFLE = 32, 64, 128, 256
 AUG_ITEM_STRIDE, AUG_OBJ_STRIDE = 25, 12
 
 
+# include/svgps.h evaluation counter layouts (float64 words)
+EVAL_GROUNDING, EVAL_OBJ_CLS, EVAL_ANSWERS = 0, 1, 2
+(EVG_ITEMS, EVG_MULTIPLE, EVG_HARD, EVG_VIEW_DEP, EVG_OG_ACC, EVG_OG_ACC_HARD, EVG_OG_ACC_VIEW_DEP, EVG_IOU25, EVG_IOU50,
+ EVG_IOU25_MULTIPLE, EVG_IOU50_MULTIPLE, EVG_TXT_ACC, EVG_OBJ) = range(13)
+EVG_SIZE = EVG_OBJ + 6
+EVO_HIT, EVO_COUNT, EVO_SIZE = 0, 1, 2
+EVA_NTYPES = 6
+EVA_ITEMS, EVA_ANS1, EVA_ANS10, EVA_TYPE_ITEMS, EVA_TYPE_ANS1, EVA_OBJ_HIT, EVA_OBJ_COUNT = 0, 1, 2, 3, 9, 15, 16
+EVA_SNAPSHOT, EVA_Q_ANS1, EVA_Q_ANS10, EVA_Q_OBJ, EVA_Q_TYPE, EVA_Q_TYPE_COUNT, EVA_SIZE = 17, 34, 35, 36, 37, 43, 49
+
+
 class AugParams(ctypes.Structure):
     _fields_ = [("flags", c_int), ("scene_rot_axis_align", c_int), ("scene_rot_shuffle", c_int),
                 ("obj_rot_axis_align", c_int), ("obj_rot_shuffle", c_int),
@@ -45,6 +56,8 @@ _POINTOPS_SIGS = {
     "sv_token_mask": [c_void_p, c_void_p, ctypes.c_longlong, c_float, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_ulonglong,
                       c_void_p, c_void_p, c_void_p],
     "sv_coin_mask": [c_void_p, ctypes.c_longlong, c_float, ctypes.c_ulonglong, c_void_p, c_void_p],
+    "sv_grounding_targets_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                 c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "sv_sa_sample_f32": [c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
                          c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
 }
@@ -148,6 +161,14 @@ _GPS_SIGS = {
                          c_void_p, c_void_p],
     "sv_attn_pool_bwd": [c_void_p, c_int, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, c_int,
                          c_void_p, c_void_p, c_int, c_void_p],
+    "sv_eval_counters_size": [c_int],
+    "sv_eval_grounding": [c_void_p, c_int, ctypes.c_longlong, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_longlong,
+                          c_void_p, c_int, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                          c_void_p],
+    "sv_eval_obj_cls": [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                        c_void_p, c_void_p],
+    "sv_eval_answers": [c_void_p, c_int, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    "sv_eval_sqa3d_batch": [c_void_p, c_void_p],
     "sv_adamw_scratch_floats": [],
     "sv_adamw_flat": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_int, c_float, c_void_p,
                       c_void_p, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p],

@@ -19,8 +19,8 @@ NVCC_FLAGS = [
 
 # library name -> sources (relative to csrc/)
 LIBS = {
-    "libsvpointops.so": ["pointops.cu", "sa_sample.cu", "fps_coop.cu", "scene_prep.cu"],
-    "libsvgps.so": ["gps_common.cu", "sa_mlp.cu", "gemm.cu", "attention.cu", "attention_bwd.cu", "pairwise_locs.cu", "cross_entropy.cu", "norm_allgather.cu", "layer_norm.cu", "colsum.cu", "train_ops.cu", "pn_train.cu", "qa_ops.cu"],
+    "libsvpointops.so": ["pointops.cu", "sa_sample.cu", "fps_coop.cu", "scene_prep.cu", "eval_targets.cu"],
+    "libsvgps.so": ["gps_common.cu", "sa_mlp.cu", "gemm.cu", "attention.cu", "attention_bwd.cu", "pairwise_locs.cu", "cross_entropy.cu", "norm_allgather.cu", "layer_norm.cu", "colsum.cu", "train_ops.cu", "pn_train.cu", "qa_ops.cu", "eval_metrics.cu"],
 }
 
 

@@ -12,21 +12,12 @@
 // Randomness is a counter hash of (seed, slot / token, k): reproducible, order-independent, nothing stored.  Sampling
 // without replacement is a keyed bijection of [0, 2^b) (xor / odd-multiply / xorshift rounds) with cycle walking onto [0, n):
 // the first P images of 0..P-1 are P distinct uniform indices — no sort, no rejection table.
+#include "counter_hash.cuh"
 #include "svcommon.h"
 
 namespace {
 
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-  x ^= x >> 33;
-  x *= 0xff51afd7ed558ccdULL;
-  x ^= x >> 33;
-  x *= 0xc4ceb9fe1a85ec53ULL;
-  x ^= x >> 33;
-  return x;
-}
-__device__ __forceinline__ unsigned hash_u32(unsigned long long seed, unsigned long long a, unsigned long long b) {
-  return (unsigned)(mix64(seed + a * 0x9E3779B97F4A7C15ULL + mix64(b + 0xD1B54A32D192ED03ULL)) >> 16);
-}
+using sv::hash_u32;
 // bijection of [0, 2^bits) keyed by (k1, k2, k3); bits >= 1
 __device__ __forceinline__ unsigned perm_pow2(unsigned x, int bits, unsigned k1, unsigned k2, unsigned k3) {
   const unsigned mask = bits >= 32 ? 0xffffffffu : ((1u << bits) - 1u);

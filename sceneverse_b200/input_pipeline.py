@@ -325,3 +325,89 @@ def build_data_dict(raw_points, slot_offsets, obj_labels, txt_ids, txt_masks, tg
     if scene_txt_ids is not None:
         d["scene_txt_ids"], d["scene_txt_masks"] = scene_txt_ids, scene_txt_masks
     return d
+
+
+def grounding_targets(points, cand_offsets, item_offsets, cand_labels, tgt_label, O, seed=0, gt_points=None, gt_offsets=None,
+                      gt_index=None, return_iou=False):
+    """Evaluation targets of a grounding batch (base.py:387-454), csrc/eval_targets.cu.
+
+    points (total, 6) f32 cuda: every candidate object's raw points; cand_offsets (n_cand + 1) int64 cuda: one CSR range per
+    candidate (>= 1 point each); item_offsets (B + 1) int64 on the HOST: the candidates of each item; cand_labels (n_cand)
+    int64 cuda; tgt_label (B,) int64 cuda.  pred mode: gt_points / gt_offsets (B + 1, cuda) hold each item's ground-truth
+    object.  gt mode: gt_index (B,) int64 cuda = the target candidate of each item (after the caller's wall / floor /
+    ceiling filter).  Returns slot_map (B, O) int32 (-1 = empty slot), tgt_object_id (B, 1), tgt_object_id_iou25 and
+    tgt_object_id_iou50 (B, O) int64 [, per-candidate IoU (n_cand,) f32]."""
+    item_offsets = torch.as_tensor(item_offsets, dtype=torch.int64).cpu()
+    B = item_offsets.numel() - 1
+    counts = item_offsets[1:] - item_offsets[:-1]
+    if B < 1 or int(item_offsets[0]) != 0 or bool((counts < 0).any()):
+        raise ValueError("item_offsets must start at 0 and be non-decreasing")
+    n_cand = int(item_offsets[-1])
+    assert points.is_cuda and points.dtype == torch.float32 and points.dim() == 2 and points.shape[1] == 6
+    assert cand_offsets.dtype == torch.int64 and cand_offsets.numel() == n_cand + 1
+    assert cand_labels.dtype == torch.int64 and cand_labels.numel() == n_cand and tgt_label.numel() == B
+    if (gt_index is None) == (gt_points is None):
+        raise ValueError("pass gt_points / gt_offsets (pred mode) or gt_index (gt mode)")
+    dev = points.device
+    slot_map = torch.empty((B, O), dtype=torch.int32, device=dev)
+    tgt = torch.empty((B, 1), dtype=torch.int64, device=dev)
+    iou25 = torch.empty((B, O), dtype=torch.int64, device=dev)
+    iou50 = torch.empty((B, O), dtype=torch.int64, device=dev)
+    iou = torch.empty(max(n_cand, 1), dtype=torch.float32, device=dev) if return_iou else None
+    cand_offsets, cand_labels, tgt_label = cand_offsets.contiguous(), cand_labels.contiguous(), tgt_label.contiguous()
+    if gt_points is not None:
+        gt_points, gt_offsets = gt_points.contiguous(), gt_offsets.contiguous()
+        assert gt_offsets.dtype == torch.int64 and gt_offsets.numel() == B + 1
+    else:
+        gt_index = gt_index.contiguous()
+        assert gt_index.dtype == torch.int64 and gt_index.numel() == B
+    lib = _lib.pointops()
+
+    def ptr(t):
+        return t.data_ptr() if t is not None else None
+
+    item_dev = item_offsets.to(dev)
+    with torch.cuda.device(dev):
+        st = lib.sv_grounding_targets_f32(points.data_ptr(), cand_offsets.data_ptr(), item_dev.data_ptr(), ptr(gt_points),
+                                          ptr(gt_offsets), ptr(gt_index), cand_labels.data_ptr(), tgt_label.data_ptr(), B, O,
+                                          int(counts.max()), int(seed) & 0x7FFFFFFFFFFFFFFF, slot_map.data_ptr(),
+                                          tgt.data_ptr(), iou25.data_ptr(), iou50.data_ptr(), ptr(iou), _stream(points))
+    _lib.check(lib, st, "sv_grounding_targets_f32")
+    out = (slot_map, tgt, iou25, iou50)
+    return out + (iou[:n_cand],) if return_iou else out
+
+
+def kept_objects(points, cand_offsets, item_offsets, slot_map):
+    """The points of the candidates `slot_map` keeps, slot by slot, and the (B*O + 1) slot_offsets over them that
+    prepare_objects / prepare_objects_aug consume (empty range = padded slot)."""
+    B, O = slot_map.shape
+    dev = points.device
+    base = torch.as_tensor(item_offsets, dtype=torch.int64)[:-1].to(dev)
+    sm = slot_map.long()
+    cand = (base[:, None] + sm.clamp(min=0)).reshape(-1)
+    starts = cand_offsets[cand]
+    lens = (cand_offsets[cand + 1] - starts) * (sm.reshape(-1) >= 0)
+    slot_offsets = torch.zeros(B * O + 1, dtype=torch.int64, device=dev)
+    slot_offsets[1:] = lens.cumsum(0)
+    total = int(slot_offsets[-1])
+    src = torch.repeat_interleave(starts - slot_offsets[:-1], lens, output_size=total) + torch.arange(total, device=dev)
+    return points[src], slot_offsets
+
+
+def build_eval_dict(points, cand_offsets, item_offsets, cand_labels, tgt_label, txt_ids, txt_masks, O, P=1024, seed=0,
+                    augment=None, gt_points=None, gt_offsets=None, gt_index=None):
+    """The evaluation batch of ScanFamilyDatasetWrapperOld (dataset_wrapper.py:147-195) on the device: the targets and crop of
+    `grounding_targets`, the kept objects processed as `augment` says (`AugSpec.from_config(cfg.data_aug, rot_aug,
+    split="val")`; None = the plain post path), boxes, no masked-LM corruption and obj_sem_masks = obj_masks."""
+    slot_map, tgt, iou25, iou50 = grounding_targets(points, cand_offsets, item_offsets, cand_labels, tgt_label, O, seed,
+                                                    gt_points, gt_offsets, gt_index)
+    kept, slot_offsets = kept_objects(points, cand_offsets, item_offsets, slot_map)
+    B = slot_map.shape[0]
+    fts, locs, masks, boxes = prepare_objects_aug(kept, slot_offsets, B, O, P, augment if augment is not None else AugSpec(),
+                                                  seed, want_boxes=True)
+    base = torch.as_tensor(item_offsets, dtype=torch.int64)[:-1].to(points.device)
+    sm = slot_map.long()
+    labels = torch.where(sm >= 0, cand_labels[(base[:, None] + sm.clamp(min=0))], torch.full_like(sm, -100))
+    return {"obj_fts": fts, "obj_locs": locs, "obj_boxes": boxes, "obj_masks": masks, "obj_sem_masks": masks.clone(),
+            "obj_labels": labels, "txt_ids": txt_ids, "txt_masks": txt_masks, "tgt_object_id": tgt,
+            "tgt_object_label": tgt_label.reshape(B, 1), "tgt_object_id_iou25": iou25, "tgt_object_id_iou50": iou50}
