@@ -83,54 +83,31 @@ int sv_linear_dgrad_bf16(const void *gy, int ldg, const void *w, int ldw, int M,
 int sv_linear_wgrad_bf16(const void *gy, int ldg, const void *x, int ldx, int M, int N, int Kin, float *dw, int ld_dw,
                          float *db, int accumulate, void *stream);
 
-/* ---- fused attention forward (wgmma): O = softmax(Q K^T * scale + spatial gate + key mask) V, head dim 64 ---------
+/* ---- fused attention (wgmma): O = softmax(Q K^T * scale + spatial gate + key mask) V, head dim 64 ------------------
  * q (B,Lq,*), k/v (B,Lk,*) bf16 with batch strides *_bs and row strides *_rs (elements, % 8 == 0); head h uses columns
  * [64h, 64h+64).  key_padding_mask (B,Lk) bytes, 1 = ignore (may be NULL).  spatial_w (B,Lq,spatial_heads*6) f32 =
  * [bias, w1..w5] per head and pairwise_locs (B,Lq,Lk,5) f32 enable the MultiHeadAttentionSpatial 'cond' gate
  * log(clamp(sigmoid(w . loc + b), 1e-6)) (reference: modules/layers/transformers.py:206-232); NULL = plain attention
- * (nn.MultiheadAttention core).  Lk <= 384.  out (B,Lq,H*64) bf16. */
-int sv_attention_fwd_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                          const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
-                          const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
-                          const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, void *stream);
-
-/* same as sv_attention_fwd_bf16, additionally storing lse (B,H,Lq) f32 = log-sum-exp of each query's logits (needed by
- * sv_attention_bwd_bf16) */
-int sv_attention_fwd_lse_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                              const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
-                              const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
-                              const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, float *lse,
-                              void *stream);
-/* Backward of the fused attention (one wgmma kernel template launched twice: dQ + gate-weight gradients with tile rows
- * == queries, dK/dV with tile rows == keys; both recompute P from Q, K, the gate and lse).  q/k/v as in the forward; o, d_o (B,Lq,H*64) bf16
- * contiguous; dq (B,Lq,H*64), dk, dv (B,Lk,H*64) bf16 contiguous; d_spatial_w (B,Lq,H*6) f32 (NULL without gate; gate
- * requires spatial_heads == H); dvec (B,H,Lq) f32 scratch.  Lq, Lk <= 384. */
-int sv_attention_bwd_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                          const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
-                          const unsigned char *key_padding_mask, const float *spatial_w, const float *pairwise_locs,
-                          const float *lse, int B, int H, int Lq, int Lk, float scale, void *dq, void *dk, void *dv,
-                          float *d_spatial_w, float *dvec, void *stream);
-
-/* Dropout variants (nn.MultiheadAttention applies dropout to the attention weights in training, reference
- * transformers.py:22-24,69-74,118-120): weight (b,h,i,j) is kept iff its 16-bit counter-based uniform (csrc/attn_common.cuh:
- * one 64-bit mix per (b,h,i) row, one 32-bit mix per key pair) >= round(p * 65536), and scaled by 1/(1-p); the backward
- * regenerates the same mask from (dropout_p, seed).  Not combinable with the spatial gate (the reference's spatial
- * attention has no weight dropout). */
+ * (nn.MultiheadAttention core).  Lk <= 384.  out (B,Lq,H*64) bf16.  lse (B,H,Lq) f32 (may be NULL) receives the
+ * log-sum-exp of each query's logits, which the backward needs.
+ * Dropout on the attention weights (nn.MultiheadAttention in training, reference transformers.py:22-24,69-74,118-120;
+ * dropout_p = 0: none): weight (b,h,i,j) is kept iff its 16-bit counter-based uniform (csrc/attn_common.cuh: one 64-bit
+ * mix per (b,h,i) row, one 32-bit mix per key pair) >= round(p * 65536), and scaled by 1/(1-p); the backward regenerates
+ * the same mask from (dropout_p, seed).  Not combinable with the spatial gate (the reference's spatial attention has no
+ * weight dropout). */
 int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
                                   const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
                                   const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
                                   const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, float *lse,
                                   float dropout_p, unsigned long long seed, void *stream);
-int sv_attention_bwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                                  const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
-                                  const unsigned char *key_padding_mask, const float *spatial_w,
-                                  const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk, float scale,
-                                  void *dq, void *dk, void *dv, float *d_spatial_w, float *dvec, float dropout_p,
-                                  unsigned long long seed, void *stream);
 
-/* same backward with strided gradient outputs: rows of dq / dk / dv are d_rs elements apart (scene stride L * d_rs), so the
- * three can be the column slices [0,E) [E,2E) [2E,3E) of ONE packed (B,L,3E) buffer — the gradient of a packed QKV
- * projection, consumed by a single dgrad / wgrad GEMM (requires Lq == Lk for a shared packed buffer) */
+/* Backward of the fused attention (one wgmma kernel template launched twice: dQ + gate-weight gradients with tile rows
+ * == queries, dK/dV with tile rows == keys; both recompute P from Q, K, the gate and lse).  q/k/v, dropout_p and seed as in
+ * the forward; o, d_o (B,Lq,H*64) bf16 contiguous; dq (B,Lq,*), dk, dv (B,Lk,*) bf16 with rows d_rs (>= H*64) elements
+ * apart (scene stride L * d_rs): d_rs = H*64 gives contiguous gradients, d_rs = 3E lets the three be the column slices
+ * [0,E) [E,2E) [2E,3E) of ONE packed (B,L,3E) buffer — the gradient of a packed QKV projection, consumed by a single
+ * dgrad / wgrad GEMM (requires Lq == Lk).  d_spatial_w (B,Lq,H*6) f32 (NULL without gate; gate requires
+ * spatial_heads == H); dvec (B,H,Lq) f32 scratch.  Lq, Lk <= 384. */
 int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
                                   const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
                                   const unsigned char *key_padding_mask, const float *spatial_w,
@@ -148,12 +125,9 @@ int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf16, int R, i
                       float eps, float dropout_p, unsigned long long seed, void *y, void *s, float *mean, float *rstd,
                       void *stream);
 /* Backward: g = dL/dy (R,D) same dtype; ds = dL/d(residual) (= dL/dx without dropout); dx = ds o mask / (1 - p) (required
- * iff dropout_p > 0); dgamma, dbeta (D) f32; scratch: sv_layer_norm_scratch_floats(D) floats (per-CTA partial sums, reduced
- * in a fixed order by a second small kernel). */
-int sv_layer_norm_bwd(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma, const float *mean,
-                      const float *rstd, float dropout_p, unsigned long long seed, void *ds, void *dx, float *dgamma,
-                      float *dbeta, float *scratch, void *stream);
-/* same; accumulate = 1 adds dgamma / dbeta into the given buffers (the flat gradient buffer) instead of overwriting them */
+ * iff dropout_p > 0); dgamma, dbeta (D) f32, overwritten (accumulate = 0) or added into (accumulate = 1: the flat gradient
+ * buffer); scratch: sv_layer_norm_scratch_floats(D) floats (per-CTA partial sums, reduced in a fixed order by a second small
+ * kernel). */
 int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma, const float *mean,
                           const float *rstd, float dropout_p, unsigned long long seed, void *ds, void *dx, float *dgamma,
                           float *dbeta, int accumulate, float *scratch, void *stream);
@@ -187,12 +161,10 @@ int sv_pairwise_locs_f32(const float *centers, int row_stride, int B, int O, flo
 
 /* Fused softmax cross-entropy, forward + gradient (reference: optim/loss/loss.py:8-9,56-61 — F.cross_entropy with
  * ignore_index): logits (R,V) bf16 (is_bf16 = 1) or f32, rows row_stride elements apart; labels (R) int64.
- * loss_rows[r] = logsumexp(row) - row[label] (0 for ignored rows); grad_logits (R,V, contiguous, same dtype, may be NULL)
- * = softmax(row) - onehot(label) (zero rows for ignored labels).  The caller divides by the number of valid rows. */
-int sv_cross_entropy_fwd_bwd(const void *logits, long long row_stride, int is_bf16, const long long *labels, int R, int V,
-                             long long ignore_index, float *loss_rows, void *grad_logits, void *stream);
-/* same, with gradient rows grad_row_stride (>= V) elements apart; columns [V, grad_row_stride) are written as zeros — the
- * gradient of a vocabulary padded to 16-byte rows (BERT LM head, V = 30522 -> 30528) feeds the backward GEMMs directly */
+ * loss_rows[r] = logsumexp(row) - row[label] (0 for ignored rows); grad_logits (R, grad_row_stride >= V, same dtype, may be
+ * NULL) = softmax(row) - onehot(label) (zero rows for ignored labels), columns [V, grad_row_stride) written as zeros — the
+ * gradient of a vocabulary padded to 16-byte rows (BERT LM head, V = 30522 -> 30528) feeds the backward GEMMs directly.
+ * The caller divides by the number of valid rows. */
 int sv_cross_entropy_fwd_bwd_strided(const void *logits, long long row_stride, int is_bf16, const long long *labels, int R,
                                      int V, long long ignore_index, float *loss_rows, void *grad_logits,
                                      long long grad_row_stride, void *stream);
@@ -300,13 +272,10 @@ int sv_pn_rowgroup_max_grad(const void *gout, const unsigned char *arg, long lon
 /* L2-normalise + all-gather fused over NVLink peer memory (reference: contra_loss.py:58-64,86-91 + dist_utils.py:131-149).
  * a, b: local (n,D) f32.  peer_bufs[world] / peer_signals[world]: DEVICE arrays of device pointers into a symmetric
  * allocation mapped on every rank: buffer = [2 parities][2 tensors][world*n][D] f32, signal = >= world uint32 words
- * (zero-initialised).  epoch must start at 1 and increase by 1 per call on every rank.  When the kernel completes the
- * local buffer holds, for parity epoch&1, normalize(a) and normalize(b) of all ranks in rank-major order. */
-int sv_normalize_allgather_f32(const float *a, const float *b, int n, int D, void *const *peer_bufs,
-                               void *const *peer_signals, unsigned *done_counter, int world, int rank, unsigned epoch,
-                               void *stream);
-/* same exchange with the epoch kept in device memory (*epoch_dev, zero-initialised, one word per exchange object): the
- * launch uses *epoch_dev + 1 and stores it back on completion, so a captured CUDA graph (frozen arguments) can replay it */
+ * (zero-initialised).  The epoch is kept in device memory (*epoch_dev, zero-initialised, one word per exchange object): the
+ * launch uses epoch = *epoch_dev + 1 and stores it back on completion, so a captured CUDA graph (frozen arguments) can replay
+ * it.  When the kernel completes the local buffer holds, for parity epoch&1, normalize(a) and normalize(b) of all ranks in
+ * rank-major order. */
 int sv_normalize_allgather_dev_f32(const float *a, const float *b, int n, int D, void *const *peer_bufs,
                                    void *const *peer_signals, unsigned *done_counter, int world, int rank,
                                    unsigned *epoch_dev, void *stream);

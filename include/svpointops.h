@@ -100,9 +100,16 @@ int sv_sa_sample_f32(const float *xyz, int B, int N, int m, float radius, int ns
  * slot).  Per slot: obj_locs (6) = [mean xyz, max-min] of the raw points; P points sampled uniformly (without replacement
  * when the object has >= P points, with replacement otherwise), centred on the SAMPLE mean, divided by the sample's max norm
  * (1 when < 1e-6), colours untouched; empty slots: all-ones points, zero locs, mask 0.  sample_idx (n_slots,P) i32 may be
- * NULL (receives the chosen raw indices, -1 for empty slots).  Randomness = counter hash of (seed, slot, k). */
-int sv_scene_prep_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int P, unsigned long long seed,
-                      float *obj_fts, float *obj_locs, unsigned char *obj_masks, int *sample_idx, void *stream);
+ * NULL (receives the chosen raw indices, -1 for empty slots).  Randomness = counter hash of (seed, slot, k).
+ * `rot_aug` (data/data_utils.py:163-178 `build_rotate_mat`): with quarter_turns (n_slots / slots_per_item) i32 in 0..3, the
+ * raw xyz of every object of item b are first rotated x @ R^T, R = [[c, -s, 0], [s, c, 0], [0, 0, 1]] in f32 with theta =
+ * quarter_turns[b] * pi / 2 (0 = not rotated); NULL = no rotation.  obj_boxes (n_slots, 6) = [(min + max) / 2, max - min] of
+ * the rotated raw points, may be NULL.  index_in (n_slots, P) i32 may be NULL (drawn from the seed) or give the sampled raw
+ * indices.  sv_quarter_turn_draw fills quarter_turns (n_items) uniformly from the seed. */
+int sv_scene_prep_rot_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int slots_per_item, int P,
+                          unsigned long long seed, const int *quarter_turns, const int *index_in, float *obj_fts,
+                          float *obj_locs, float *obj_boxes, unsigned char *obj_masks, int *sample_idx, void *stream);
+int sv_quarter_turn_draw(int n_items, unsigned long long seed, int *quarter_turns, void *stream);
 /* Training-split object augmentation (the `data_aug` configs): restates data/datasets/data_augmentor.py
  * `DataAugmentor.update_data_dict` followed by data/datasets/base.py:742-776 `_obj_processing_aug`, per object slot, in this
  * order: scene flip of all raw xyz; scene scaling about the raw mean (taken after the flip); subsample P points (without
@@ -153,17 +160,6 @@ int sv_scene_prep_aug_f32(const float *raw_points, const long long *slot_offsets
                           const sv_aug_params *params, const double *item_tab, const double *obj_tab, const int *index_in,
                           const float *noise_in, unsigned long long seed, float *obj_fts, float *obj_locs, float *obj_boxes,
                           unsigned char *obj_masks, int *index_out, float *noise_out, void *stream);
-/* `_obj_processing_post` with `rot_aug` (data/datasets/base.py:697-741, data/data_utils.py:163-178 `build_rotate_mat`): the
- * raw xyz of every object of item b are first rotated x @ R^T, R = [[c, -s, 0], [s, c, 0], [0, 0, 1]] in f32 with theta =
- * quarter_turns[b] * pi / 2 (0 = not rotated), then processed exactly as sv_scene_prep_f32 does.  quarter_turns (n_slots /
- * slots_per_item) i32 in 0..3 may be NULL (no rotation: then obj_fts / obj_locs / obj_masks / sample_idx equal
- * sv_scene_prep_f32's for the same seed).  obj_boxes (n_slots, 6) = [(min + max) / 2, max - min] of the rotated raw points, may
- * be NULL.  index_in (n_slots, P) i32 may be NULL (drawn from the seed as in sv_scene_prep_f32) or give the sampled raw indices.
- * sv_quarter_turn_draw fills quarter_turns (n_items) uniformly from the seed. */
-int sv_scene_prep_rot_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int slots_per_item, int P,
-                          unsigned long long seed, const int *quarter_turns, const int *index_in, float *obj_fts,
-                          float *obj_locs, float *obj_boxes, unsigned char *obj_masks, int *sample_idx, void *stream);
-int sv_quarter_turn_draw(int n_items, unsigned long long seed, int *quarter_turns, void *stream);
 /* BERT masked-LM corruption (data/data_utils.py:76-104 `random_word`): for tokens with attention_mask != 0, with probability
  * mask_ratio the label is the original id and the token becomes [MASK] (80 %), a uniform random id (10 %) or stays (10 %);
  * every other label is -1.  ids / attention_mask / out_ids / labels: (n_tokens) int64. */

@@ -1,9 +1,14 @@
-"""ctypes binding of libsvpointops (include/svpointops.h).  No fallback: if the CUDA library is
-missing or a call fails this raises — the product path never routes around the native code."""
+"""ctypes binding of libsvpointops and libsvgps.  Argument and return types come from the headers the libraries are built
+against (include/svpointops.h, include/svgps.h).  No fallback: if the CUDA library is missing or a call fails this raises —
+the product path never routes around the native code."""
 import ctypes
 import os
+import re
+
+import torch
 
 _LIBDIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "lib")
+_INCLUDE = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include")
 _cache = {}
 
 c_int, c_float, c_void_p = ctypes.c_int, ctypes.c_float, ctypes.c_void_p
@@ -33,36 +38,6 @@ class AugParams(ctypes.Structure):
                 ("obj_trans", ctypes.c_double * 3), ("obj_rot", ctypes.c_double * 3), ("jitter", ctypes.c_double)]
 
 
-_POINTOPS_SIGS = {
-    # name: argtypes
-    "sv_fps_f32": [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "sv_gather_points_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_gather_points_grad_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_ball_query_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p],
-    "sv_group_points_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_group_points_grad_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_three_nn_f32": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "sv_three_interpolate_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_three_interpolate_grad_f32": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_fps_ballquery_f32": [c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_scene_prep_f32": [c_void_p, c_void_p, c_int, c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_scene_prep_rot_f32": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p,
-                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_quarter_turn_draw": [c_int, ctypes.c_ulonglong, c_void_p, c_void_p],
-    "sv_aug_draw": [ctypes.POINTER(AugParams), c_int, c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p],
-    "sv_scene_prep_aug_f32": [c_void_p, c_void_p, c_int, c_int, c_int, ctypes.POINTER(AugParams), c_void_p, c_void_p, c_void_p,
-                              c_void_p, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                              c_void_p],
-    "sv_token_mask": [c_void_p, c_void_p, ctypes.c_longlong, c_float, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_ulonglong,
-                      c_void_p, c_void_p, c_void_p],
-    "sv_coin_mask": [c_void_p, ctypes.c_longlong, c_float, ctypes.c_ulonglong, c_void_p, c_void_p],
-    "sv_grounding_targets_f32": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                 c_int, ctypes.c_ulonglong, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_sa_sample_f32": [c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
-                         c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p],
-}
-
-
 class NativeLibraryError(RuntimeError):
     pass
 
@@ -80,134 +55,90 @@ def _load(name):
     return lib
 
 
+# C type -> ctypes type of every non-pointer parameter and return type the headers use; any other type is an error
+_CTYPES = {"int": c_int, "unsigned": ctypes.c_uint, "float": c_float, "double": ctypes.c_double,
+           "long long": ctypes.c_longlong, "unsigned long long": ctypes.c_ulonglong}
+_PROTOTYPE = re.compile(r"([\w\s*]+?)\b(\w+)\s*\(([^()]*)\)")
+_PARAM = re.compile(r"([\w\s*]*?)\s*\b(\w+)")
+
+
+def _ctype(decl, fn, is_return):
+    """The ctypes type of one C declaration without its name ("const float *", "unsigned long long")."""
+    base = " ".join(w for w in decl.replace("*", " ").split() if w != "const")
+    if "*" in decl:
+        if base == "sv_aug_params" and not is_return:
+            return ctypes.POINTER(AugParams)
+        if base == "char" and is_return:
+            return ctypes.c_char_p
+        return c_void_p
+    if base in _CTYPES:
+        return _CTYPES[base]
+    raise NativeLibraryError(f"{fn}: no ctypes mapping for the C type '{decl.strip()}'")
+
+
+def parse_prototypes(text):
+    """{name: (restype, argtypes)} of every prototype `ret name(params);` of a C header, after comments, preprocessor lines
+    and `extern "C" {` are stripped.  Statements without parentheses (typedefs, enums) are skipped."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    text = re.sub(r"^[ \t]*#[^\n]*", " ", text, flags=re.M)
+    text = re.sub(r'extern\s+"C"\s*\{', " ", text)
+    protos = {}
+    for stmt in text.split(";"):
+        if "(" not in stmt:
+            continue
+        m = _PROTOTYPE.fullmatch(stmt.strip())
+        if m is None:
+            raise NativeLibraryError(f"not a prototype: '{' '.join(stmt.split())}'")
+        ret, name, params = m.groups()
+        argtypes = []
+        if params.strip() != "void":
+            for param in params.split(","):
+                pm = _PARAM.fullmatch(param.strip())
+                if pm is None:
+                    raise NativeLibraryError(f"{name}: cannot parse the parameter '{' '.join(param.split())}'")
+                argtypes.append(_ctype(pm.group(1), name, False))
+        protos[name] = (_ctype(ret, name, True), argtypes)
+    return protos
+
+
+def _bind(lib, header):
+    """Sets argtypes / restype of every function `header` (include/) declares."""
+    with open(os.path.join(_INCLUDE, header)) as f:
+        protos = parse_prototypes(f.read())
+    for name, (restype, argtypes) in protos.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
+
+
 def pointops():
     lib = _load("libsvpointops.so")
     if not getattr(lib, "_sv_ready", False):
-        for fn, argtypes in _POINTOPS_SIGS.items():
-            f = getattr(lib, fn)
-            f.argtypes = argtypes
-            f.restype = c_int
-        lib.sv_version.restype = c_int
-        lib.sv_status_string.restype = ctypes.c_char_p
-        lib.sv_status_string.argtypes = [c_int]
-        lib.sv_last_cuda_error.restype = c_int
-        lib.sv_last_cuda_error_string.restype = ctypes.c_char_p
-        lib.sv_launch_count.restype = ctypes.c_ulonglong
+        _bind(lib, "svpointops.h")
         lib._sv_ready = True
     return lib
-
-
-_GPS_SIGS = {
-    "sv_gemm_bf16": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int,
-                     c_int, c_int, c_void_p],
-    "sv_gemm_bf16_ex": [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
-                        c_void_p, c_int, c_int, c_int, c_void_p],
-    "sv_attention_fwd_bf16": [c_void_p, ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p,
-                              ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_int,
-                              c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p],
-    "sv_pairwise_locs_f32": [c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p],
-    "sv_cross_entropy_fwd_bwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, ctypes.c_longlong, c_void_p,
-                                 c_void_p, c_void_p],
-    "sv_cross_entropy_fwd_bwd_strided": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, ctypes.c_longlong,
-                                         c_void_p, c_void_p, ctypes.c_longlong, c_void_p],
-    "sv_normalize_allgather_f32": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                   ctypes.c_uint, c_void_p],
-    "sv_normalize_allgather_dev_f32": [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int,
-                                       c_void_p, c_void_p],
-    "sv_attention_fwd_lse_bf16": [c_void_p, ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p,
-                                  ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_int,
-                                  c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p],
-    "sv_attention_bwd_bf16": [c_void_p, ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p,
-                              ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
-                              c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_attention_fwd_dropout_bf16": [c_void_p, ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p,
-                                      ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p,
-                                      c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_float,
-                                      ctypes.c_ulonglong, c_void_p],
-    "sv_attention_bwd_dropout_bf16": [c_void_p, ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p,
-                                      ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_float, ctypes.c_ulonglong, c_void_p],
-    "sv_attention_bwd_strided_bf16": [c_void_p, ctypes.c_longlong, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p,
-                                      ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                      c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p,
-                                      c_void_p, c_float, ctypes.c_ulonglong, c_void_p],
-    "sv_layer_norm_fwd": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_float, ctypes.c_ulonglong,
-                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_layer_norm_bwd": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, ctypes.c_ulonglong,
-                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_layer_norm_bwd_acc": [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_float, ctypes.c_ulonglong,
-                              c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
-    "sv_layer_norm_scratch_floats": [c_int],
-    "sv_dropout_seed_offset": [c_void_p],
-    "sv_colsum": [c_void_p, ctypes.c_longlong, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "sv_colsum_scratch_floats": [c_int],
-    "sv_l2norm_fwd": [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p],
-    "sv_l2norm_bwd": [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p],
-    "sv_gemm_force_ctas": [c_int],
-    "sv_gemm_profile": [c_void_p],
-    "sv_linear_fwd_bf16": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_float, ctypes.c_ulonglong,
-                           c_void_p, c_int, c_int, c_void_p, c_void_p],
-    "sv_linear_dgrad_bf16": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_float,
-                             ctypes.c_ulonglong, c_void_p, c_int, c_int, c_void_p],
-    "sv_linear_wgrad_bf16": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p],
-    "sv_act_bwd_bf16": [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p],
-    "sv_embedding_bwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, ctypes.c_longlong, ctypes.c_longlong,
-                         c_void_p, c_void_p],
-    "sv_scale_inplace": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p],
-    "sv_bce_logits_fwd_bwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
-                              c_void_p, c_void_p, ctypes.c_longlong, c_void_p],
-    "sv_attn_pool_fwd": [c_void_p, c_int, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, c_int, c_void_p,
-                         c_void_p, c_void_p],
-    "sv_attn_pool_bwd": [c_void_p, c_int, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_int, c_int, c_int,
-                         c_void_p, c_void_p, c_int, c_void_p],
-    "sv_eval_counters_size": [c_int],
-    "sv_eval_grounding": [c_void_p, c_int, ctypes.c_longlong, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_longlong,
-                          c_void_p, c_int, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                          c_void_p],
-    "sv_eval_obj_cls": [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
-                        c_void_p, c_void_p],
-    "sv_eval_answers": [c_void_p, c_int, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
-    "sv_eval_sqa3d_batch": [c_void_p, c_void_p],
-    "sv_adamw_scratch_floats": [],
-    "sv_adamw_flat": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_int, c_float, c_void_p,
-                      c_void_p, c_float, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p],
-    "sv_pn_group_rows": [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_pn_group_rows_grad": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_pn_scratch_floats": [c_int],
-    "sv_pn_bn_relu_fwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
-                          c_void_p, c_void_p],
-    "sv_pn_bn_relu_bwd": [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                          c_void_p, c_int, c_void_p, c_void_p],
-    "sv_pn_sync_floats": [c_int, c_int],
-    "sv_pn_bn_sync_push": [c_int, c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                           c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p],
-    "sv_pn_bn_sync_finish_fwd": [c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p,
-                                 c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_pn_bn_sync_finish_bwd": [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                 c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_pn_rowgroup_max": [c_void_p, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p],
-    "sv_pn_rowgroup_max_grad": [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p],
-    "sv_sa_mlp_param_bytes": [c_int],
-    "sv_sa1_mlp_bf16": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
-    "sv_sa2_mlp_bf16": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p],
-}
 
 
 def gps():
     lib = _load("libsvgps.so")
     if not getattr(lib, "_sv_ready", False):
-        for fn, argtypes in _GPS_SIGS.items():
-            f = getattr(lib, fn)
-            f.argtypes = argtypes
-            f.restype = c_int
-        lib.svgps_launch_count.restype = ctypes.c_ulonglong
-        lib.svgps_last_cuda_error_string.restype = ctypes.c_char_p
+        _bind(lib, "svgps.h")
         # status strings live in libsvpointops
         lib.sv_status_string = pointops().sv_status_string
         lib.sv_last_cuda_error_string = lib.svgps_last_cuda_error_string
         lib._sv_ready = True
     return lib
+
+
+def ptr(t):
+    """The device pointer of tensor `t`, or NULL for None."""
+    return None if t is None else t.data_ptr()
+
+
+def call(lib, name, device, *args):
+    """lib.name(*args, stream) under `device`, with that device's current stream appended; raises if the status is not 0."""
+    with torch.cuda.device(device):
+        st = getattr(lib, name)(*args, torch.cuda.current_stream(device).cuda_stream)
+    check(lib, st, name)
 
 
 def check(lib, status, what):

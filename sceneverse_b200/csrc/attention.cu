@@ -223,25 +223,6 @@ int launch_fwd(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &
 
 }  // namespace
 
-extern "C" int sv_attention_fwd_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                                     const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
-                                     const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
-                                     const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale,
-                                     void *stream) {
-  return sv_attention_fwd_dropout_bf16(q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, out, o_bs, o_rs, key_padding_mask,
-                                       spatial_w, spatial_heads, pairwise_locs, B, H, Lq, Lk, scale, nullptr, 0.f, 0ull,
-                                       stream);
-}
-
-extern "C" int sv_attention_fwd_lse_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                                         const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
-                                         const unsigned char *key_padding_mask, const float *spatial_w,
-                                         int spatial_heads, const float *pairwise_locs, int B, int H, int Lq, int Lk,
-                                         float scale, float *lse, void *stream) {
-  return sv_attention_fwd_dropout_bf16(q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, out, o_bs, o_rs, key_padding_mask,
-                                       spatial_w, spatial_heads, pairwise_locs, B, H, Lq, Lk, scale, lse, 0.f, 0ull, stream);
-}
-
 extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
                                              int k_rs, const void *v, long long v_bs, int v_rs, void *out, long long o_bs,
                                              int o_rs, const unsigned char *key_padding_mask, const float *spatial_w,

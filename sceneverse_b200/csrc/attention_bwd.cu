@@ -333,29 +333,6 @@ int launch_both(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap 
 
 }  // namespace
 
-extern "C" int sv_attention_bwd_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                                     const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
-                                     const unsigned char *key_padding_mask, const float *spatial_w,
-                                     const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk,
-                                     float scale, void *dq, void *dk, void *dv, float *d_spatial_w, float *dvec,
-                                     void *stream) {
-  return sv_attention_bwd_dropout_bf16(q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, o, d_o, key_padding_mask, spatial_w,
-                                       pairwise_locs, lse, B, H, Lq, Lk, scale, dq, dk, dv, d_spatial_w, dvec, 0.f, 0ull,
-                                       stream);
-}
-
-extern "C" int sv_attention_bwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
-                                             int k_rs, const void *v, long long v_bs, int v_rs, const void *o,
-                                             const void *d_o, const unsigned char *key_padding_mask,
-                                             const float *spatial_w, const float *pairwise_locs, const float *lse, int B,
-                                             int H, int Lq, int Lk, float scale, void *dq, void *dk, void *dv,
-                                             float *d_spatial_w, float *dvec, float dropout_p, unsigned long long seed,
-                                             void *stream) {
-  return sv_attention_bwd_strided_bf16(q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, o, d_o, key_padding_mask, spatial_w,
-                                       pairwise_locs, lse, B, H, Lq, Lk, scale, dq, dk, dv, H * attn::DH, d_spatial_w, dvec,
-                                       dropout_p, seed, stream);
-}
-
 extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
                                              int k_rs, const void *v, long long v_bs, int v_rs, const void *o,
                                              const void *d_o, const unsigned char *key_padding_mask,

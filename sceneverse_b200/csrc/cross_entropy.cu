@@ -65,13 +65,6 @@ __global__ void __launch_bounds__(256) ce_fwd_bwd_kernel(const T *__restrict__ l
 
 }  // namespace
 
-extern "C" int sv_cross_entropy_fwd_bwd(const void *logits, long long row_stride, int is_bf16, const long long *labels,
-                                        int R, int V, long long ignore_index, float *loss_rows, void *grad_logits,
-                                        void *stream) {
-  return sv_cross_entropy_fwd_bwd_strided(logits, row_stride, is_bf16, labels, R, V, ignore_index, loss_rows, grad_logits,
-                                          V, stream);
-}
-
 extern "C" int sv_cross_entropy_fwd_bwd_strided(const void *logits, long long row_stride, int is_bf16,
                                                 const long long *labels, int R, int V, long long ignore_index,
                                                 float *loss_rows, void *grad_logits, long long grad_row_stride,

@@ -432,12 +432,6 @@ extern "C" int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf1
   }
 }
 
-extern "C" int sv_layer_norm_bwd(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma,
-                                 const float *mean, const float *rstd, float dropout_p, unsigned long long seed, void *ds,
-                                 void *dx, float *dgamma, float *dbeta, float *scratch, void *stream) {
-  return sv_layer_norm_bwd_acc(g, s, io_bf16, R, D, gamma, mean, rstd, dropout_p, seed, ds, dx, dgamma, dbeta, 0, scratch, stream);
-}
-
 extern "C" int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma,
                                      const float *mean, const float *rstd, float dropout_p, unsigned long long seed, void *ds,
                                      void *dx, float *dgamma, float *dbeta, int accumulate, float *scratch, void *stream) {

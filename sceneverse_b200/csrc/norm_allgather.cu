@@ -17,7 +17,6 @@ struct NagArgs {
   unsigned *const *peer_sig; // [world] device pointers to signal words (flag[src_rank] at index src_rank)
   unsigned *done_counter;    // local, zero-initialised, reset by the last CTA
   int n, D, world, rank;
-  unsigned epoch;            // >= 1, increases by one per call on every rank (used when epoch_dev is null)
   unsigned *epoch_dev;       // device-resident epoch: this launch uses *epoch_dev + 1 and stores it back when done
 };
 
@@ -26,7 +25,7 @@ __global__ void __launch_bounds__(256) norm_allgather_kernel(const NagArgs g) {
   __shared__ unsigned is_last, s_epoch;
   // a captured CUDA graph freezes by-value arguments, so the epoch can live on the device: every CTA reads it before it
   // arrives on the done counter, the last CTA advances it after the exchange
-  if (threadIdx.x == 0) s_epoch = g.epoch_dev != nullptr ? *reinterpret_cast<volatile unsigned *>(g.epoch_dev) + 1u : g.epoch;
+  if (threadIdx.x == 0) s_epoch = *reinterpret_cast<volatile unsigned *>(g.epoch_dev) + 1u;
   __syncthreads();
   const unsigned epoch = s_epoch;
   const int row = blockIdx.x % g.n, t = blockIdx.x / g.n;  // t = 0: tensor a, 1: tensor b
@@ -67,22 +66,11 @@ __global__ void __launch_bounds__(256) norm_allgather_kernel(const NagArgs g) {
   __syncthreads();
   if (threadIdx.x == 0) {
     *g.done_counter = 0u;
-    if (g.epoch_dev != nullptr) *g.epoch_dev = epoch;
+    *g.epoch_dev = epoch;
   }
 }
 
 }  // namespace
-
-extern "C" int sv_normalize_allgather_f32(const float *a, const float *b, int n, int D, void *const *peer_bufs,
-                                          void *const *peer_signals, unsigned *done_counter, int world, int rank,
-                                          unsigned epoch, void *stream) {
-  if (n < 0 || D < 1 || world < 1 || world > 64 || rank < 0 || rank >= world || epoch == 0) return SV_ERR_INVALID_ARG;
-  if (n == 0) return SV_OK;
-  if (!a || !b || !peer_bufs || !peer_signals || !done_counter) return SV_ERR_INVALID_ARG;
-  NagArgs g{a, b, (float *const *)peer_bufs, (unsigned *const *)peer_signals, done_counter, n, D, world, rank, epoch, nullptr};
-  norm_allgather_kernel<<<2 * n, 256, 0, (cudaStream_t)stream>>>(g);
-  return sv::after_launch();
-}
 
 extern "C" int sv_normalize_allgather_dev_f32(const float *a, const float *b, int n, int D, void *const *peer_bufs,
                                               void *const *peer_signals, unsigned *done_counter, int world, int rank,
@@ -90,7 +78,7 @@ extern "C" int sv_normalize_allgather_dev_f32(const float *a, const float *b, in
   if (n < 0 || D < 1 || world < 1 || world > 64 || rank < 0 || rank >= world) return SV_ERR_INVALID_ARG;
   if (n == 0) return SV_OK;
   if (!a || !b || !peer_bufs || !peer_signals || !done_counter || !epoch_dev) return SV_ERR_INVALID_ARG;
-  NagArgs g{a, b, (float *const *)peer_bufs, (unsigned *const *)peer_signals, done_counter, n, D, world, rank, 0u, epoch_dev};
+  NagArgs g{a, b, (float *const *)peer_bufs, (unsigned *const *)peer_signals, done_counter, n, D, world, rank, epoch_dev};
   norm_allgather_kernel<<<2 * n, 256, 0, (cudaStream_t)stream>>>(g);
   return sv::after_launch();
 }

@@ -40,7 +40,6 @@ struct PrepArgs {
   float *locs;                 // (S, 6)
   unsigned char *masks;        // (S) 1 = real object
   int *sample_idx;             // (S, P) or null: the chosen raw indices (tests)
-  // rotated post path (scene_prep_kernel<true> only)
   int slots_per_item;
   const int *quarter_turns;    // (S / slots_per_item) or null: x @ R^T per item, theta = k pi / 2
   const int *index_in;         // (S, P) or null: given raw indices instead of drawn ones
@@ -86,9 +85,8 @@ __device__ __forceinline__ QuarterTurn quarter_turn(int k) {
                 : QuarterTurn{(float)-1.8369701987210297e-16, -1.f};
 }
 
-// kExt = false: sv_scene_prep_f32, unchanged.  kExt = true: sv_scene_prep_rot_f32 (optional per-item quarter turn of the raw
-// points, optional given indices, optional boxes).
-template <bool kExt>
+// `_obj_processing_post` per object slot, with an optional per-item quarter turn of the raw points, optional given indices and
+// optional boxes.
 __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
   extern __shared__ __align__(16) float pts[];   // [P][6] sampled points
   __shared__ double redd[8];
@@ -99,7 +97,7 @@ __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
   if (n <= 0) {   // padded slot: all-ones points (dataset_wrapper.py:62-64), zero locs, mask 0
     for (int i = tid; i < a.P * 6; i += 256) out[i] = 1.0f;
     if (tid < 6) a.locs[(size_t)s * 6 + tid] = 0.f;
-    if (kExt && a.boxes != nullptr && tid < 6) a.boxes[(size_t)s * 6 + tid] = 0.f;
+    if (a.boxes != nullptr && tid < 6) a.boxes[(size_t)s * 6 + tid] = 0.f;
     if (tid == 0) a.masks[s] = 0;
     if (a.sample_idx != nullptr)
       for (int i = tid; i < a.P; i += 256) a.sample_idx[(size_t)s * a.P + i] = -1;
@@ -108,7 +106,7 @@ __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
   const float *raw = a.raw + (size_t)beg * 6;
   bool rot = false;
   QuarterTurn R{1.f, 0.f};
-  if (kExt && a.quarter_turns != nullptr) {
+  if (a.quarter_turns != nullptr) {
     const int k = a.quarter_turns[s / a.slots_per_item] & 3;
     rot = k != 0;   // theta = 0: build_rotate_mat returns None, the points are left as they are
     if (rot) R = quarter_turn(k);
@@ -118,7 +116,7 @@ __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
   float mnx = INFINITY, mny = INFINITY, mnz = INFINITY, mxx = -INFINITY, mxy = -INFINITY, mxz = -INFINITY;
   for (long long i = tid; i < n; i += 256) {
     float x = raw[i * 6], y = raw[i * 6 + 1], z = raw[i * 6 + 2];
-    if (kExt && rot) R.apply(x, y, z);
+    if (rot) R.apply(x, y, z);
     sx += x; sy += y; sz += z;
     mnx = fminf(mnx, x); mny = fminf(mny, y); mnz = fminf(mnz, z);
     mxx = fmaxf(mxx, x); mxy = fmaxf(mxy, y); mxz = fmaxf(mxz, z);
@@ -130,7 +128,7 @@ __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
     float *l = a.locs + (size_t)s * 6;
     l[0] = (float)(sx / (double)n); l[1] = (float)(sy / (double)n); l[2] = (float)(sz / (double)n);
     l[3] = mxx - mnx; l[4] = mxy - mny; l[5] = mxz - mnz;
-    if (kExt && a.boxes != nullptr) {   // base.py:714-718: box centre = (max + min) / 2, size = max - min
+    if (a.boxes != nullptr) {   // base.py:714-718: box centre = (max + min) / 2, size = max - min
       float *bx = a.boxes + (size_t)s * 6;
       bx[0] = (mxx + mnx) / 2; bx[1] = (mxy + mny) / 2; bx[2] = (mxz + mnz) / 2;
       bx[3] = l[3]; bx[4] = l[4]; bx[5] = l[5];
@@ -145,7 +143,7 @@ __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
   double cx = 0, cy = 0, cz = 0;
   for (int k = tid; k < a.P; k += 256) {
     long long idx;
-    if (kExt && a.index_in != nullptr) {
+    if (a.index_in != nullptr) {
       idx = a.index_in[(size_t)s * a.P + k];
     } else if (n < a.P) {   // with replacement
       idx = (long long)(((unsigned long long)hash_u32(a.seed, (unsigned long long)s, 16 + (unsigned long long)k) * (unsigned long long)n) >> 32);
@@ -158,7 +156,7 @@ __global__ void __launch_bounds__(256) scene_prep_kernel(const PrepArgs a) {
     const float *p = raw + idx * 6;
 #pragma unroll
     for (int c = 0; c < 6; ++c) pts[k * 6 + c] = p[c];
-    if (kExt && rot) {
+    if (rot) {
       R.apply(pts[k * 6], pts[k * 6 + 1], pts[k * 6 + 2]);
       cx += pts[k * 6]; cy += pts[k * 6 + 1]; cz += pts[k * 6 + 2];
     } else {
@@ -501,22 +499,6 @@ __global__ void __launch_bounds__(256) coin_mask_kernel(const unsigned char *val
 
 }  // namespace
 
-extern "C" int sv_scene_prep_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int P,
-                                 unsigned long long seed, float *obj_fts, float *obj_locs, unsigned char *obj_masks,
-                                 int *sample_idx, void *stream) {
-  if (n_slots < 0 || P < 1 || P > 8192) return SV_ERR_INVALID_ARG;
-  if (n_slots == 0) return SV_OK;
-  if (!raw_points || !slot_offsets || !obj_fts || !obj_locs || !obj_masks) return SV_ERR_INVALID_ARG;
-  const size_t smem = (size_t)P * 6 * sizeof(float);
-  if (smem > 48 * 1024) {
-    int rc = sv::cuda_status(cudaFuncSetAttribute(scene_prep_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (rc) return rc;
-  }
-  PrepArgs a{raw_points, slot_offsets, n_slots, P, seed, obj_fts, obj_locs, obj_masks, sample_idx, 1, nullptr, nullptr, nullptr};
-  scene_prep_kernel<false><<<n_slots, 256, smem, (cudaStream_t)stream>>>(a);
-  return sv::after_launch();
-}
-
 extern "C" int sv_scene_prep_rot_f32(const float *raw_points, const long long *slot_offsets, int n_slots, int slots_per_item,
                                      int P, unsigned long long seed, const int *quarter_turns, const int *index_in,
                                      float *obj_fts, float *obj_locs, float *obj_boxes, unsigned char *obj_masks,
@@ -526,12 +508,12 @@ extern "C" int sv_scene_prep_rot_f32(const float *raw_points, const long long *s
   if (!raw_points || !slot_offsets || !obj_fts || !obj_locs || !obj_masks) return SV_ERR_INVALID_ARG;
   const size_t smem = (size_t)P * 6 * sizeof(float);
   if (smem > 48 * 1024) {
-    int rc = sv::cuda_status(cudaFuncSetAttribute(scene_prep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int rc = sv::cuda_status(cudaFuncSetAttribute(scene_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (rc) return rc;
   }
   PrepArgs a{raw_points, slot_offsets, n_slots, P, seed, obj_fts, obj_locs, obj_masks, sample_idx, slots_per_item, quarter_turns,
              index_in, obj_boxes};
-  scene_prep_kernel<true><<<n_slots, 256, smem, (cudaStream_t)stream>>>(a);
+  scene_prep_kernel<<<n_slots, 256, smem, (cudaStream_t)stream>>>(a);
   return sv::after_launch();
 }
 

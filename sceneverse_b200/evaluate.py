@@ -19,10 +19,6 @@ from . import _lib
 __all__ = ["ScanReferEval", "ReferIt3DEval", "ScanQAEval", "SQA3DEval", "PretrainObjEval", "EvalRunner"]
 
 
-def _stream(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def _is_bf16(t):
     if t.dtype not in (torch.bfloat16, torch.float32):
         raise TypeError(f"logits must be bf16 or f32, got {t.dtype}")
@@ -46,10 +42,6 @@ def _bytes(t):
     if t is None:
         return None
     return (t if t.dtype in (torch.bool, torch.uint8) else t.bool()).contiguous()
-
-
-def _ptr(t):
-    return t.data_ptr() if t is not None else None
 
 
 def _save_flag(cfg):
@@ -81,11 +73,8 @@ def _launch_obj_cls(tensors, data_dict, valid, counters):
     bf = arr(ctypes.c_int, [_is_bf16(t) for t in tensors])
     rs = arr(ctypes.c_longlong, [t.stride(1) for t in tensors])
     its = arr(ctypes.c_longlong, [t.stride(0) for t in tensors])
-    lib = _lib.gps()
-    with torch.cuda.device(labels.device):
-        st = lib.sv_eval_obj_cls(n, ptrs, bf, rs, its, B, O, C, labels.data_ptr(), masks.data_ptr(), _ptr(valid),
-                                 counters.data_ptr(), _stream(labels))
-    _lib.check(lib, st, "sv_eval_obj_cls")
+    _lib.call(_lib.gps(), "sv_eval_obj_cls", labels.device, n, ptrs, bf, rs, its, B, O, C, labels.data_ptr(), masks.data_ptr(),
+              _lib.ptr(valid), counters.data_ptr())
 
 
 class _CounterEvaluator:
@@ -177,14 +166,11 @@ class _GroundingEval(_CounterEvaluator):
         # ScanRefer splits by is_multiple, ReferIt3D by is_hard and is_view_dependent
         split_keys = ("is_multiple",) if self.uses_iou else ("is_hard", "is_view_dependent")
         flags = [_bytes(data_dict.get(k)) if k in split_keys else None for k in ("is_multiple", "is_hard", "is_view_dependent")]
-        lib = _lib.gps()
-        with torch.cuda.device(og.device):
-            st = lib.sv_eval_grounding(og.data_ptr(), _is_bf16(og), og.stride(0), og.stride(1), B, O, tgt.data_ptr(), _ptr(iou25), _ptr(iou50),
-                                       iou25.stride(0) if iou25 is not None else 0, _ptr(txt),
-                                       _is_bf16(txt) if txt is not None else 0, txt.stride(0) if txt is not None else 0,
-                                       txt.shape[1] if txt is not None else 0, _ptr(label), *[_ptr(f) for f in flags],
-                                       _ptr(valid), counters.data_ptr(), _stream(og))
-        _lib.check(lib, st, "sv_eval_grounding")
+        _lib.call(_lib.gps(), "sv_eval_grounding", og.device, og.data_ptr(), _is_bf16(og), og.stride(0), og.stride(1), B, O,
+                  tgt.data_ptr(), _lib.ptr(iou25), _lib.ptr(iou50), iou25.stride(0) if iou25 is not None else 0, _lib.ptr(txt),
+                  _is_bf16(txt) if txt is not None else 0, txt.stride(0) if txt is not None else 0,
+                  txt.shape[1] if txt is not None else 0, _lib.ptr(label), *[_lib.ptr(f) for f in flags], _lib.ptr(valid),
+                  counters.data_ptr())
         keys = _obj_logit_keys(data_dict)
         if len(keys) > 3:
             raise NotImplementedError(f"at most three object logits tensors, got {keys}")
@@ -251,11 +237,8 @@ def _launch_answers(data_dict, valid, counters, with_type):
     if tuple(label.shape) != (B, A):
         raise ValueError(f"answer_label must be {(B, A)}, got {tuple(label.shape)}")
     qtype = _i64(data_dict["sqa_type"], "sqa_type").reshape(-1) if with_type else None
-    lib = _lib.gps()
-    with torch.cuda.device(s.device):
-        st = lib.sv_eval_answers(s.data_ptr(), _is_bf16(s), s.stride(0), B, A, label.data_ptr(), _ptr(qtype), _ptr(valid),
-                                 counters.data_ptr(), _stream(s))
-    _lib.check(lib, st, "sv_eval_answers")
+    _lib.call(_lib.gps(), "sv_eval_answers", s.device, s.data_ptr(), _is_bf16(s), s.stride(0), B, A, label.data_ptr(),
+              _lib.ptr(qtype), _lib.ptr(valid), counters.data_ptr())
 
 
 class ScanQAEval(_CounterEvaluator):
@@ -317,10 +300,7 @@ class SQA3DEval(_CounterEvaluator):
     def _launch(self, data_dict, valid, counters):
         _launch_answers(data_dict, valid, counters, with_type=True)
         _launch_obj_cls([data_dict["obj_cls_raw_logits"]], data_dict, valid, counters[_lib.EVA_OBJ_HIT:])
-        lib = _lib.gps()
-        with torch.cuda.device(counters.device):
-            st = lib.sv_eval_sqa3d_batch(counters.data_ptr(), _stream(counters))
-        _lib.check(lib, st, "sv_eval_sqa3d_batch")
+        _lib.call(_lib.gps(), "sv_eval_sqa3d_batch", counters.device, counters.data_ptr())
 
     def batch_metrics(self, data_dict):
         c = self._batch_counts(data_dict)

@@ -46,12 +46,9 @@ class FusedNormGather:
         a = a.detach().float().contiguous()
         b = b.detach().float().contiguous()
         assert a.shape == (self.n, self.D) and b.shape == (self.n, self.D)
-        lib = _lib.gps()
-        with torch.cuda.device(a.device):
-            st = lib.sv_normalize_allgather_dev_f32(a.data_ptr(), b.data_ptr(), self.n, self.D, self.peer_bufs.data_ptr(),
-                                                    self.peer_sigs.data_ptr(), self.done.data_ptr(), self.world, self.rank,
-                                                    self.epoch_dev.data_ptr(), torch.cuda.current_stream(a.device).cuda_stream)
-        _lib.check(lib, st, "sv_normalize_allgather_dev_f32")
+        _lib.call(_lib.gps(), "sv_normalize_allgather_dev_f32", a.device, a.data_ptr(), b.data_ptr(), self.n, self.D,
+                  self.peer_bufs.data_ptr(), self.peer_sigs.data_ptr(), self.done.data_ptr(), self.world, self.rank,
+                  self.epoch_dev.data_ptr())
         wn = self.world * self.n
         parity = (self.epoch_dev & 1).long()          # the kernel stored the epoch it used; stream-ordered after it
         out = self.buf[:self.data_floats].view(2, 2, wn, self.D).index_select(0, parity)[0]

@@ -20,10 +20,6 @@ import torch
 from . import _lib
 
 
-def _stream(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def prepare_objects(raw_points, slot_offsets, B, O, P=1024, seed=0, return_indices=False):
     """raw_points (total,6) f32 cuda, slot_offsets (B*O+1) int64 cuda -> obj_fts (B,O,P,6) f32, obj_locs (B,O,6) f32,
     obj_masks (B,O) bool [, sample indices (B,O,P) i32]."""
@@ -35,12 +31,10 @@ def prepare_objects(raw_points, slot_offsets, B, O, P=1024, seed=0, return_indic
     locs = torch.empty((B, O, 6), dtype=torch.float32, device=dev)
     masks = torch.empty((B, O), dtype=torch.uint8, device=dev)
     idx = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_indices else None
-    lib = _lib.pointops()
-    with torch.cuda.device(dev):
-        st = lib.sv_scene_prep_f32(raw_points.data_ptr(), slot_offsets.data_ptr(), B * O, P, int(seed) & 0x7FFFFFFFFFFFFFFF,
-                                   fts.data_ptr(), locs.data_ptr(), masks.data_ptr(),
-                                   idx.data_ptr() if idx is not None else None, _stream(raw_points))
-    _lib.check(lib, st, "sv_scene_prep_f32")
+    # the post path without quarter turns; slots_per_item >= 1 keeps a batch without object slots (O = 0) valid
+    _lib.call(_lib.pointops(), "sv_scene_prep_rot_f32", dev, raw_points.data_ptr(), slot_offsets.data_ptr(), B * O, max(O, 1),
+              P, int(seed) & 0x7FFFFFFFFFFFFFFF, None, None, fts.data_ptr(), locs.data_ptr(), None, masks.data_ptr(),
+              _lib.ptr(idx))
     out = (fts, locs, masks.bool())
     return out + (idx,) if return_indices else out
 
@@ -228,52 +222,46 @@ def prepare_objects_aug(raw_points, slot_offsets, B, O, P, spec, seed, want_boxe
     seed = int(seed) & 0x7FFFFFFFFFFFFFFF
     lib = _lib.pointops()
 
-    def ptr(t):
-        return t.data_ptr() if t is not None else None
-
     def given(key, shape, dtype):
         t = draws.get(key)
         if t is None or tuple(t.shape) != shape or t.dtype != dtype or t.device != dev:
             raise ValueError(f"draws[{key!r}] must be a {dtype} tensor of shape {shape} on {dev}")
         return t.contiguous()
 
-    st = _stream(raw_points)
-    with torch.cuda.device(dev):
-        if spec.path == "post":
-            if draws is not None:
-                qt, idx_in = given("quarter_turns", (B,), torch.int32), given("index", (B, O, P), torch.int32)
-            else:
-                qt, idx_in = None, None
-                if spec.rot_aug:
-                    qt = torch.empty(B, dtype=torch.int32, device=dev)
-                    _lib.check(lib, lib.sv_quarter_turn_draw(B, seed, qt.data_ptr(), st), "sv_quarter_turn_draw")
-            idx_out = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_draws else None
-            rc = lib.sv_scene_prep_rot_f32(raw_points.data_ptr(), slot_offsets.data_ptr(), B * O, O, P, seed, ptr(qt), ptr(idx_in),
-                                           fts.data_ptr(), locs.data_ptr(), ptr(boxes), masks.data_ptr(), ptr(idx_out), st)
-            _lib.check(lib, rc, "sv_scene_prep_rot_f32")
-            used = {"quarter_turns": qt if qt is not None else torch.zeros(B, dtype=torch.int32, device=dev),
-                    "index": idx_out}
+    if spec.path == "post":
+        if draws is not None:
+            qt, idx_in = given("quarter_turns", (B,), torch.int32), given("index", (B, O, P), torch.int32)
         else:
-            params = spec.params()
-            jitter = spec.jitter is not None
-            if draws is not None:
-                item, obj = given("item", (B, _lib.AUG_ITEM_STRIDE), torch.float64), given("obj", (B, O, _lib.AUG_OBJ_STRIDE), torch.float64)
-                idx_in = given("index", (B, O, P), torch.int32)
-                noise_in = given("noise", (B, O, P, 3), torch.float32) if jitter else None
-            else:
-                item = torch.empty((B, _lib.AUG_ITEM_STRIDE), dtype=torch.float64, device=dev)
-                obj = torch.empty((B, O, _lib.AUG_OBJ_STRIDE), dtype=torch.float64, device=dev)
-                idx_in = noise_in = None
-                _lib.check(lib, lib.sv_aug_draw(params, B, O, seed, item.data_ptr(), obj.data_ptr(), st), "sv_aug_draw")
-            idx_out = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_draws else None
-            noise_out = torch.empty((B, O, P, 3), dtype=torch.float32, device=dev) if return_draws and jitter else None
-            rc = lib.sv_scene_prep_aug_f32(raw_points.data_ptr(), slot_offsets.data_ptr(), B, O, P, params, item.data_ptr(),
-                                           obj.data_ptr(), ptr(idx_in), ptr(noise_in), seed, fts.data_ptr(), locs.data_ptr(),
-                                           ptr(boxes), masks.data_ptr(), ptr(idx_out), ptr(noise_out), st)
-            _lib.check(lib, rc, "sv_scene_prep_aug_f32")
-            used = {"item": item, "obj": obj, "index": idx_out}
-            if jitter:
-                used["noise"] = noise_out
+            qt, idx_in = None, None
+            if spec.rot_aug:
+                qt = torch.empty(B, dtype=torch.int32, device=dev)
+                _lib.call(lib, "sv_quarter_turn_draw", dev, B, seed, qt.data_ptr())
+        idx_out = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_draws else None
+        _lib.call(lib, "sv_scene_prep_rot_f32", dev, raw_points.data_ptr(), slot_offsets.data_ptr(), B * O, O, P, seed,
+                  _lib.ptr(qt), _lib.ptr(idx_in), fts.data_ptr(), locs.data_ptr(), _lib.ptr(boxes), masks.data_ptr(),
+                  _lib.ptr(idx_out))
+        used = {"quarter_turns": qt if qt is not None else torch.zeros(B, dtype=torch.int32, device=dev),
+                "index": idx_out}
+    else:
+        params = spec.params()
+        jitter = spec.jitter is not None
+        if draws is not None:
+            item, obj = given("item", (B, _lib.AUG_ITEM_STRIDE), torch.float64), given("obj", (B, O, _lib.AUG_OBJ_STRIDE), torch.float64)
+            idx_in = given("index", (B, O, P), torch.int32)
+            noise_in = given("noise", (B, O, P, 3), torch.float32) if jitter else None
+        else:
+            item = torch.empty((B, _lib.AUG_ITEM_STRIDE), dtype=torch.float64, device=dev)
+            obj = torch.empty((B, O, _lib.AUG_OBJ_STRIDE), dtype=torch.float64, device=dev)
+            idx_in = noise_in = None
+            _lib.call(lib, "sv_aug_draw", dev, params, B, O, seed, item.data_ptr(), obj.data_ptr())
+        idx_out = torch.empty((B, O, P), dtype=torch.int32, device=dev) if return_draws else None
+        noise_out = torch.empty((B, O, P, 3), dtype=torch.float32, device=dev) if return_draws and jitter else None
+        _lib.call(lib, "sv_scene_prep_aug_f32", dev, raw_points.data_ptr(), slot_offsets.data_ptr(), B, O, P, params,
+                  item.data_ptr(), obj.data_ptr(), _lib.ptr(idx_in), _lib.ptr(noise_in), seed, fts.data_ptr(), locs.data_ptr(),
+                  _lib.ptr(boxes), masks.data_ptr(), _lib.ptr(idx_out), _lib.ptr(noise_out))
+        used = {"item": item, "obj": obj, "index": idx_out}
+        if jitter:
+            used["noise"] = noise_out
     out = (fts, locs, masks.bool())
     if want_boxes:
         out += (boxes,)
@@ -285,11 +273,8 @@ def mask_tokens(txt_ids, txt_masks, mask_ratio=0.15, mask_token_id=103, vocab_si
     assert txt_ids.is_cuda and txt_ids.dtype == torch.int64 and txt_masks.dtype == torch.int64 and txt_ids.shape == txt_masks.shape
     ids, am = txt_ids.contiguous(), txt_masks.contiguous()
     out, lab = torch.empty_like(ids), torch.empty_like(ids)
-    lib = _lib.pointops()
-    with torch.cuda.device(ids.device):
-        st = lib.sv_token_mask(ids.data_ptr(), am.data_ptr(), ids.numel(), float(mask_ratio), int(mask_token_id), int(vocab_size),
-                               int(seed) & 0x7FFFFFFFFFFFFFFF, out.data_ptr(), lab.data_ptr(), _stream(ids))
-    _lib.check(lib, st, "sv_token_mask")
+    _lib.call(_lib.pointops(), "sv_token_mask", ids.device, ids.data_ptr(), am.data_ptr(), ids.numel(), float(mask_ratio),
+              int(mask_token_id), int(vocab_size), int(seed) & 0x7FFFFFFFFFFFFFFF, out.data_ptr(), lab.data_ptr())
     return out, lab
 
 
@@ -297,10 +282,8 @@ def mask_objects(obj_masks, drop_ratio=0.1, seed=0):
     """random_point_cloud: (B,O) bool -> (B,O) bool, True = keep the object's semantic features."""
     v = obj_masks.to(torch.uint8).contiguous()
     out = torch.empty_like(v)
-    lib = _lib.pointops()
-    with torch.cuda.device(v.device):
-        st = lib.sv_coin_mask(v.data_ptr(), v.numel(), float(drop_ratio), int(seed) & 0x7FFFFFFFFFFFFFFF, out.data_ptr(), _stream(v))
-    _lib.check(lib, st, "sv_coin_mask")
+    _lib.call(_lib.pointops(), "sv_coin_mask", v.device, v.data_ptr(), v.numel(), float(drop_ratio),
+              int(seed) & 0x7FFFFFFFFFFFFFFF, out.data_ptr())
     return out.bool()
 
 
@@ -361,18 +344,11 @@ def grounding_targets(points, cand_offsets, item_offsets, cand_labels, tgt_label
     else:
         gt_index = gt_index.contiguous()
         assert gt_index.dtype == torch.int64 and gt_index.numel() == B
-    lib = _lib.pointops()
-
-    def ptr(t):
-        return t.data_ptr() if t is not None else None
-
     item_dev = item_offsets.to(dev)
-    with torch.cuda.device(dev):
-        st = lib.sv_grounding_targets_f32(points.data_ptr(), cand_offsets.data_ptr(), item_dev.data_ptr(), ptr(gt_points),
-                                          ptr(gt_offsets), ptr(gt_index), cand_labels.data_ptr(), tgt_label.data_ptr(), B, O,
-                                          int(counts.max()), int(seed) & 0x7FFFFFFFFFFFFFFF, slot_map.data_ptr(),
-                                          tgt.data_ptr(), iou25.data_ptr(), iou50.data_ptr(), ptr(iou), _stream(points))
-    _lib.check(lib, st, "sv_grounding_targets_f32")
+    _lib.call(_lib.pointops(), "sv_grounding_targets_f32", dev, points.data_ptr(), cand_offsets.data_ptr(), item_dev.data_ptr(),
+              _lib.ptr(gt_points), _lib.ptr(gt_offsets), _lib.ptr(gt_index), cand_labels.data_ptr(), tgt_label.data_ptr(), B, O,
+              int(counts.max()), int(seed) & 0x7FFFFFFFFFFFFFFF, slot_map.data_ptr(), tgt.data_ptr(), iou25.data_ptr(),
+              iou50.data_ptr(), _lib.ptr(iou))
     out = (slot_map, tgt, iou25, iou50)
     return out + (iou[:n_cand],) if return_iou else out
 

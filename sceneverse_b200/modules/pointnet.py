@@ -209,15 +209,12 @@ class PointNetPP(nn.Module):
         sa1, sa2 = self.encoder[0], self.encoder[1]
         fi1, nx1, bi1, fi2, nx2, bi2 = _ext.sa_sample2(xyz, sa1.npoint, sa1.radius, sa1.nsample,
                                                        sa2.npoint, sa2.radius, sa2.nsample)
-        lib = _lib.gps()
-        st = torch.cuda.current_stream(pts.device).cuda_stream
         feat1 = torch.empty((B, 32, 128), dtype=torch.bfloat16, device=pts.device)
-        _lib.check(lib, lib.sv_sa1_mlp_bf16(pts.data_ptr(), nx1.data_ptr(), bi1.data_ptr(), pk["sa1"].data_ptr(), B, P,
-                                            sa1.nsample, feat1.data_ptr(), st), "sv_sa1_mlp_bf16")
+        _lib.call(_lib.gps(), "sv_sa1_mlp_bf16", pts.device, pts.data_ptr(), nx1.data_ptr(), bi1.data_ptr(), pk["sa1"].data_ptr(),
+                  B, P, sa1.nsample, feat1.data_ptr())
         feat2 = torch.empty((B, 16, 256), dtype=torch.bfloat16, device=pts.device)
-        _lib.check(lib, lib.sv_sa2_mlp_bf16(nx1.data_ptr(), feat1.data_ptr(), nx2.data_ptr(), bi2.data_ptr(),
-                                            pk["sa2"].data_ptr(), B, 32, sa2.nsample, feat2.data_ptr(), st),
-                   "sv_sa2_mlp_bf16")
+        _lib.call(_lib.gps(), "sv_sa2_mlp_bf16", pts.device, nx1.data_ptr(), feat1.data_ptr(), nx2.data_ptr(), bi2.data_ptr(),
+                  pk["sa2"].data_ptr(), B, 32, sa2.nsample, feat2.data_ptr())
         # SA3 (GroupAll over the 16 points: 259->256->512->768, BN folded, ReLU, max over the points) + fc, as four
         # wgmma GEMMs with fused shift/ReLU (and row-group max) epilogues.  xyz is NOT centred here (GroupAll,
         # pointnet2_utils.py:389-419).

@@ -18,14 +18,8 @@ def gemm(a, w, bias=None, act=None, residual=None, out_dtype=torch.bfloat16, row
         bias = bias.float().contiguous()
     if residual is not None:
         residual = residual.to(out_dtype).contiguous()
-    lib = _lib.gps()
-    with torch.cuda.device(a.device):
-        st = lib.sv_gemm_bf16(a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), M, N, K,
-                              bias.data_ptr() if bias is not None else None, _ACT[act],
-                              residual.data_ptr() if residual is not None else None, out.data_ptr(), N,
-                              1 if out_dtype == torch.float32 else 0, rowmax,
-                              torch.cuda.current_stream(a.device).cuda_stream)
-    _lib.check(lib, st, "sv_gemm_bf16")
+    _lib.call(_lib.gps(), "sv_gemm_bf16", a.device, a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), M, N, K,
+              _lib.ptr(bias), _ACT[act], _lib.ptr(residual), out.data_ptr(), N, 1 if out_dtype == torch.float32 else 0, rowmax)
     return out
 
 
@@ -55,15 +49,10 @@ def attention(q, k, v, num_heads, key_padding_mask=None, spatial_w=None, spatial
         sw = spatial_w.float().contiguous()
         locs = pairwise_locs.float().contiguous()
     lse = torch.empty((B, num_heads, Lq), dtype=torch.float32, device=q.device) if return_lse else None
-    lib = _lib.gps()
-    with torch.cuda.device(q.device):
-        st = lib.sv_attention_fwd_dropout_bf16(
-            q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
-            v.stride(1), out.data_ptr(), out.stride(0), out.stride(1), kpm.data_ptr() if kpm is not None else None,
-            sw.data_ptr() if sw is not None else None, int(spatial_heads), locs.data_ptr() if locs is not None else None,
-            B, num_heads, Lq, Lk, 0.125, lse.data_ptr() if lse is not None else None, float(dropout_p), int(seed),
-            torch.cuda.current_stream(q.device).cuda_stream)
-    _lib.check(lib, st, "sv_attention_fwd_dropout_bf16")
+    _lib.call(_lib.gps(), "sv_attention_fwd_dropout_bf16", q.device,
+              q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
+              v.stride(1), out.data_ptr(), out.stride(0), out.stride(1), _lib.ptr(kpm), _lib.ptr(sw), int(spatial_heads),
+              _lib.ptr(locs), B, num_heads, Lq, Lk, 0.125, _lib.ptr(lse), float(dropout_p), int(seed))
     return (out, lse) if return_lse else out
 
 
@@ -92,16 +81,11 @@ def attention_backward(q, k, v, out, grad_out, lse, num_heads, key_padding_mask=
     if spatial_w is not None:
         sw, locs = spatial_w.float().contiguous(), pairwise_locs.float().contiguous()
         dsw = torch.empty_like(sw)
-    lib = _lib.gps()
-    with torch.cuda.device(dev):
-        st = lib.sv_attention_bwd_strided_bf16(
-            q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
-            v.stride(1), out.data_ptr(), grad_out.data_ptr(), kpm.data_ptr() if kpm is not None else None,
-            sw.data_ptr() if sw is not None else None, locs.data_ptr() if locs is not None else None, lse.data_ptr(),
-            B, num_heads, Lq, Lk, 0.125, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), d_rs,
-            dsw.data_ptr() if dsw is not None else None, dvec.data_ptr(), float(dropout_p), int(seed),
-            torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(lib, st, "sv_attention_bwd_strided_bf16")
+    _lib.call(_lib.gps(), "sv_attention_bwd_strided_bf16", dev,
+              q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
+              v.stride(1), out.data_ptr(), grad_out.data_ptr(), _lib.ptr(kpm), _lib.ptr(sw), _lib.ptr(locs), lse.data_ptr(),
+              B, num_heads, Lq, Lk, 0.125, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), d_rs, _lib.ptr(dsw), dvec.data_ptr(),
+              float(dropout_p), int(seed))
     return dq, dk, dv, dsw
 
 
@@ -112,10 +96,8 @@ def colsum(x):
     lib = _lib.gps()
     out = torch.empty(N, dtype=torch.float32, device=x.device)
     scratch = torch.empty(lib.sv_colsum_scratch_floats(N), dtype=torch.float32, device=x.device)
-    with torch.cuda.device(x.device):
-        st = lib.sv_colsum(x.data_ptr(), x.stride(0), 1 if x.dtype == torch.bfloat16 else 0, R, N, out.data_ptr(),
-                           scratch.data_ptr(), torch.cuda.current_stream(x.device).cuda_stream)
-    _lib.check(lib, st, "sv_colsum")
+    _lib.call(lib, "sv_colsum", x.device, x.data_ptr(), x.stride(0), 1 if x.dtype == torch.bfloat16 else 0, R, N, out.data_ptr(),
+              scratch.data_ptr())
     return out
 
 
@@ -130,18 +112,10 @@ def gemm_ex(a, b, a_transposed=False, b_transposed=False, bias=None, act=None, o
     out = torch.empty((M, N), dtype=out_dtype, device=a.device)
     if bias is not None:
         bias = bias.float().contiguous()
-    lib = _lib.gps()
-    with torch.cuda.device(a.device):
-        st = lib.sv_gemm_bf16_ex(a.data_ptr(), a.stride(0), 1 if a_transposed else 0, b.data_ptr(), b.stride(0),
-                                 1 if b_transposed else 0, M, N, K, bias.data_ptr() if bias is not None else None, _ACT[act],
-                                 None, out.data_ptr(), N, 1 if out_dtype == torch.float32 else 0, 0,
-                                 torch.cuda.current_stream(a.device).cuda_stream)
-    _lib.check(lib, st, "sv_gemm_bf16_ex")
+    _lib.call(_lib.gps(), "sv_gemm_bf16_ex", a.device, a.data_ptr(), a.stride(0), 1 if a_transposed else 0, b.data_ptr(),
+              b.stride(0), 1 if b_transposed else 0, M, N, K, _lib.ptr(bias), _ACT[act], None, out.data_ptr(), N,
+              1 if out_dtype == torch.float32 else 0, 0)
     return out
-
-
-def _stream(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
 
 
 def _rows_ok(t):
@@ -160,13 +134,9 @@ def linear_fwd(x, w, bias=None, act=None, dropout_p=0.0, seed=0, out_dtype=torch
     pre = torch.empty_like(out) if want_pre else None
     if bias is not None:
         assert bias.dtype == torch.float32 and bias.is_contiguous()
-    lib = _lib.gps()
-    with torch.cuda.device(x.device):
-        st = lib.sv_linear_fwd_bf16(x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), M, N, K,
-                                    bias.data_ptr() if bias is not None else None, _ACT[act], float(dropout_p), int(seed),
-                                    out.data_ptr(), out.stride(0), 1 if out.dtype == torch.float32 else 0,
-                                    pre.data_ptr() if pre is not None else None, _stream(x))
-    _lib.check(lib, st, "sv_linear_fwd_bf16")
+    _lib.call(_lib.gps(), "sv_linear_fwd_bf16", x.device, x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), M, N, K,
+              _lib.ptr(bias), _ACT[act], float(dropout_p), int(seed), out.data_ptr(), out.stride(0),
+              1 if out.dtype == torch.float32 else 0, _lib.ptr(pre))
     return (out, pre) if want_pre else out
 
 
@@ -179,13 +149,9 @@ def linear_dgrad(g, w, act=None, aux=None, dropout_p=0.0, seed=0, n_red=None, ou
     dx = torch.empty((M, Kin), dtype=out_dtype, device=g.device)
     if aux is not None:
         assert aux.dtype == torch.bfloat16 and aux.shape == (M, Kin) and aux.stride(1) == 1
-    lib = _lib.gps()
-    with torch.cuda.device(g.device):
-        st = lib.sv_linear_dgrad_bf16(g.data_ptr(), g.stride(0), w.data_ptr(), w.stride(0), M, N, Kin, _ACT[act],
-                                      aux.data_ptr() if aux is not None else None, aux.stride(0) if aux is not None else 0,
-                                      float(dropout_p), int(seed), dx.data_ptr(), dx.stride(0),
-                                      1 if out_dtype == torch.float32 else 0, _stream(g))
-    _lib.check(lib, st, "sv_linear_dgrad_bf16")
+    _lib.call(_lib.gps(), "sv_linear_dgrad_bf16", g.device, g.data_ptr(), g.stride(0), w.data_ptr(), w.stride(0), M, N, Kin,
+              _ACT[act], _lib.ptr(aux), aux.stride(0) if aux is not None else 0, float(dropout_p), int(seed), dx.data_ptr(),
+              dx.stride(0), 1 if out_dtype == torch.float32 else 0)
     return dx
 
 
@@ -202,12 +168,8 @@ def linear_wgrad(g, x, n_out=None, dw=None, db=None, want_db=False, accumulate=F
         assert not accumulate
         db = torch.empty(N, dtype=torch.float32, device=g.device)
     assert dw.dtype == torch.float32 and dw.stride(1) == 1 and dw.shape == (N, Kin)
-    lib = _lib.gps()
-    with torch.cuda.device(g.device):
-        st = lib.sv_linear_wgrad_bf16(g.data_ptr(), g.stride(0), x.data_ptr(), x.stride(0), M, N, Kin, dw.data_ptr(),
-                                      dw.stride(0), db.data_ptr() if db is not None else None, 1 if accumulate else 0,
-                                      _stream(g))
-    _lib.check(lib, st, "sv_linear_wgrad_bf16")
+    _lib.call(_lib.gps(), "sv_linear_wgrad_bf16", g.device, g.data_ptr(), g.stride(0), x.data_ptr(), x.stride(0), M, N, Kin,
+              dw.data_ptr(), dw.stride(0), _lib.ptr(db), 1 if accumulate else 0)
     return dw, db
 
 
@@ -215,11 +177,8 @@ def act_bwd(g, aux, act):
     """g * act'(aux): (M,N) bf16; relu: aux = forward output, gelu: aux = pre-activation."""
     assert g.dtype == torch.bfloat16 and aux.dtype == torch.bfloat16 and g.shape == aux.shape and _rows_ok(g) and _rows_ok(aux)
     out = torch.empty((g.shape[0], g.shape[1]), dtype=torch.bfloat16, device=g.device)
-    lib = _lib.gps()
-    with torch.cuda.device(g.device):
-        st = lib.sv_act_bwd_bf16(g.data_ptr(), g.stride(0), aux.data_ptr(), aux.stride(0), _ACT[act], g.shape[0], g.shape[1],
-                                 out.data_ptr(), out.stride(0), _stream(g))
-    _lib.check(lib, st, "sv_act_bwd_bf16")
+    _lib.call(_lib.gps(), "sv_act_bwd_bf16", g.device, g.data_ptr(), g.stride(0), aux.data_ptr(), aux.stride(0), _ACT[act],
+              g.shape[0], g.shape[1], out.data_ptr(), out.stride(0))
     return out
 
 
@@ -232,12 +191,8 @@ def embedding_bwd(grad_out, ids, dw, padding_idx=-1):
     ids = ids.reshape(-1).contiguous()
     assert ids.dtype == torch.int64 and dw.dtype == torch.float32 and dw.is_contiguous() and dw.shape[1] == D
     assert g2.dtype in (torch.bfloat16, torch.float32) and g2.shape[0] == ids.numel()
-    lib = _lib.gps()
-    with torch.cuda.device(g2.device):
-        st = lib.sv_embedding_bwd(g2.data_ptr(), g2.stride(0), 1 if g2.dtype == torch.bfloat16 else 0, ids.data_ptr(),
-                                  ids.numel(), D, dw.shape[0], int(padding_idx if padding_idx is not None else -1),
-                                  dw.data_ptr(), _stream(g2))
-    _lib.check(lib, st, "sv_embedding_bwd")
+    _lib.call(_lib.gps(), "sv_embedding_bwd", g2.device, g2.data_ptr(), g2.stride(0), 1 if g2.dtype == torch.bfloat16 else 0,
+              ids.data_ptr(), ids.numel(), D, dw.shape[0], int(padding_idx if padding_idx is not None else -1), dw.data_ptr())
     return dw
 
 

@@ -461,12 +461,8 @@ def calc_pairwise_locs(obj_centers, obj_whls, eps=1e-10, pairwise_rel_type='cent
         from . import _lib
         B, O, _ = obj_centers.shape
         out = torch.empty((B, O, O, 5), dtype=torch.float32, device=obj_centers.device)
-        lib = _lib.gps()
-        with torch.cuda.device(obj_centers.device):
-            st = lib.sv_pairwise_locs_f32(obj_centers.data_ptr(), obj_centers.stride(1), B, O, float(eps),
-                                          1 if spatial_dist_norm else 0, out.data_ptr(),
-                                          torch.cuda.current_stream(obj_centers.device).cuda_stream)
-        _lib.check(lib, st, "sv_pairwise_locs_f32")
+        _lib.call(_lib.gps(), "sv_pairwise_locs_f32", obj_centers.device, obj_centers.data_ptr(), obj_centers.stride(1), B, O,
+                  float(eps), 1 if spatial_dist_norm else 0, out.data_ptr())
         return out
     d = obj_centers[:, :, None, :] - obj_centers[:, None, :, :]
     dist = torch.sqrt((d ** 2).sum(3) + eps)
@@ -563,13 +559,9 @@ class _CrossEntropyFn(torch.autograd.Function):
         loss_rows = torch.empty(R, dtype=torch.float32, device=logits2d.device)
         need_grad = logits2d.requires_grad
         grad = torch.empty((R, W), dtype=logits2d.dtype, device=logits2d.device) if need_grad else None
-        lib = _lib.gps()
-        with torch.cuda.device(logits2d.device):
-            st = lib.sv_cross_entropy_fwd_bwd_strided(
-                logits2d.data_ptr(), logits2d.stride(0), 1 if logits2d.dtype == torch.bfloat16 else 0, labels.data_ptr(), R,
-                V, int(ignore_index), loss_rows.data_ptr(), grad.data_ptr() if grad is not None else None, W,
-                torch.cuda.current_stream(logits2d.device).cuda_stream)
-        _lib.check(lib, st, "sv_cross_entropy_fwd_bwd_strided")
+        _lib.call(_lib.gps(), "sv_cross_entropy_fwd_bwd_strided", logits2d.device, logits2d.data_ptr(), logits2d.stride(0),
+                  1 if logits2d.dtype == torch.bfloat16 else 0, labels.data_ptr(), R, V, int(ignore_index), loss_rows.data_ptr(),
+                  _lib.ptr(grad), W)
         # same validity predicate as the kernel: a label outside [0, V) that is not ignore_index contributes nothing
         count = ((labels != ignore_index) & (labels >= 0) & (labels < V)).sum().float()
         ctx.save_for_backward(grad, count)
@@ -579,22 +571,24 @@ class _CrossEntropyFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout):
         grad, count = ctx.saved_tensors
-        # the (R, V) gradient (195 MB for the LM head) is scaled IN PLACE: one pass instead of a second 195 MB tensor; a
-        # second backward through the same node (retain_graph) would scale it twice, so it is refused
-        if ctx.scaled:
-            raise RuntimeError("ops.cross_entropy: backward through the same graph twice is not supported (the saved "
-                               "gradient buffer is consumed in place)")
-        ctx.scaled = True
-        scale = (gout.float() / count).reshape(1).contiguous()
-        if grad.is_contiguous() and grad.numel() % 8 == 0 and grad.data_ptr() % 16 == 0:
-            from . import _lib
-            lib = _lib.gps()
-            with torch.cuda.device(grad.device):
-                st = lib.sv_scale_inplace(grad.data_ptr(), grad.numel(), 1 if grad.dtype == torch.bfloat16 else 0,
-                                          scale.data_ptr(), torch.cuda.current_stream(grad.device).cuda_stream)
-            _lib.check(lib, st, "sv_scale_inplace")
-            return grad, None, None, None
-        return grad.mul_(scale.to(grad.dtype)), None, None, None
+        return _scale_saved_grad(ctx, "cross_entropy", grad, gout, count), None, None, None
+
+
+def _scale_saved_grad(ctx, what, grad, gout, divisor):
+    """grad *= gout / divisor for the gradient a fused loss forward saved.  The (R, V) gradient (195 MB for the LM head) is
+    scaled IN PLACE: one pass instead of a second tensor of that size; a second backward through the same node
+    (retain_graph) would scale it twice, so it is refused."""
+    if ctx.scaled:
+        raise RuntimeError(f"ops.{what}: backward through the same graph twice is not supported (the saved "
+                           "gradient buffer is consumed in place)")
+    ctx.scaled = True
+    scale = (gout.float() / divisor).reshape(1).contiguous()
+    if grad.is_contiguous() and grad.numel() % 8 == 0 and grad.data_ptr() % 16 == 0:
+        from . import _lib
+        _lib.call(_lib.gps(), "sv_scale_inplace", grad.device, grad.data_ptr(), grad.numel(),
+                  1 if grad.dtype == torch.bfloat16 else 0, scale.data_ptr())
+        return grad
+    return grad.mul_(scale.to(grad.dtype))
 
 
 _BCE_COUNTERS = {}
@@ -621,14 +615,9 @@ class _BCEWithLogitsFn(torch.autograd.Function):
         loss_rows = torch.empty(R, dtype=torch.float32, device=dev)
         loss = torch.empty((), dtype=torch.float32, device=dev)
         grad = torch.empty((R, W), dtype=logits2d.dtype, device=dev) if logits2d.requires_grad else None
-        lib = _lib.gps()
-        with torch.cuda.device(dev):
-            st = lib.sv_bce_logits_fwd_bwd(
-                logits2d.data_ptr(), logits2d.stride(0), 1 if logits2d.dtype == torch.bfloat16 else 0, labels2d.data_ptr(),
-                weight_u8.data_ptr() if weight_u8 is not None else None, R, n_classes, loss_rows.data_ptr(), loss.data_ptr(),
-                _bce_counter(dev).data_ptr(), grad.data_ptr() if grad is not None else None, W,
-                torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(lib, st, "sv_bce_logits_fwd_bwd")
+        _lib.call(_lib.gps(), "sv_bce_logits_fwd_bwd", dev, logits2d.data_ptr(), logits2d.stride(0),
+                  1 if logits2d.dtype == torch.bfloat16 else 0, labels2d.data_ptr(), _lib.ptr(weight_u8), R, n_classes,
+                  loss_rows.data_ptr(), loss.data_ptr(), _bce_counter(dev).data_ptr(), _lib.ptr(grad), W)
         ctx.save_for_backward(grad)
         ctx.rows, ctx.scaled = R, False
         return loss
@@ -636,20 +625,7 @@ class _BCEWithLogitsFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gout):
         (grad,) = ctx.saved_tensors
-        if ctx.scaled:
-            raise RuntimeError("ops.bce_with_logits_sum: backward through the same graph twice is not supported (the saved "
-                               "gradient buffer is consumed in place)")
-        ctx.scaled = True
-        scale = (gout.float() / ctx.rows).reshape(1).contiguous()
-        if grad.is_contiguous() and grad.numel() % 8 == 0 and grad.data_ptr() % 16 == 0:
-            from . import _lib
-            lib = _lib.gps()
-            with torch.cuda.device(grad.device):
-                st = lib.sv_scale_inplace(grad.data_ptr(), grad.numel(), 1 if grad.dtype == torch.bfloat16 else 0,
-                                          scale.data_ptr(), torch.cuda.current_stream(grad.device).cuda_stream)
-            _lib.check(lib, st, "sv_scale_inplace")
-            return grad, None, None, None
-        return grad.mul_(scale.to(grad.dtype)), None, None, None
+        return _scale_saved_grad(ctx, "bce_with_logits_sum", grad, gout, ctx.rows), None, None, None
 
 
 def bce_with_logits_sum(logits, labels, weight=None):
@@ -685,12 +661,8 @@ class _AttentionPoolFn(torch.autograd.Function):
         B, L, D = x.shape
         p = torch.empty((B, L), dtype=torch.float32, device=x.device)
         pooled = torch.empty((B, D), dtype=torch.bfloat16, device=x.device)
-        lib = _lib.gps()
-        with torch.cuda.device(x.device):
-            st = lib.sv_attn_pool_fwd(scores.data_ptr(), scores.shape[-1], x.data_ptr(), x.stride(0), x.stride(1),
-                                      pad_mask_u8.data_ptr() if pad_mask_u8 is not None else None, B, L, D, p.data_ptr(),
-                                      pooled.data_ptr(), torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(lib, st, "sv_attn_pool_fwd")
+        _lib.call(_lib.gps(), "sv_attn_pool_fwd", x.device, scores.data_ptr(), scores.shape[-1], x.data_ptr(), x.stride(0),
+                  x.stride(1), _lib.ptr(pad_mask_u8), B, L, D, p.data_ptr(), pooled.data_ptr())
         ctx.save_for_backward(x, p, pad_mask_u8)
         ctx.score_w = scores.shape[-1]
         return pooled
@@ -705,12 +677,8 @@ class _AttentionPoolFn(torch.autograd.Function):
             g = g.contiguous()
         dx = torch.empty((B, L, D), dtype=torch.bfloat16, device=x.device)
         dscore = torch.empty((B, L, ctx.score_w), dtype=torch.bfloat16, device=x.device)
-        lib = _lib.gps()
-        with torch.cuda.device(x.device):
-            st = lib.sv_attn_pool_bwd(g.data_ptr(), g.stride(0), p.data_ptr(), x.data_ptr(), x.stride(0), x.stride(1),
-                                      mask.data_ptr() if mask is not None else None, B, L, D, dx.data_ptr(), dscore.data_ptr(),
-                                      ctx.score_w, torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(lib, st, "sv_attn_pool_bwd")
+        _lib.call(_lib.gps(), "sv_attn_pool_bwd", x.device, g.data_ptr(), g.stride(0), p.data_ptr(), x.data_ptr(), x.stride(0),
+                  x.stride(1), _lib.ptr(mask), B, L, D, dx.data_ptr(), dscore.data_ptr(), ctx.score_w)
         return dscore, dx, None
 
 
@@ -773,14 +741,9 @@ class _LayerNormFn(torch.autograd.Function):
         y = torch.empty_like(x2)
         s = torch.empty_like(x2) if need_s else None
         stats = torch.empty((2, R), dtype=torch.float32, device=x.device)
-        lib = _lib.gps()
-        with torch.cuda.device(x.device):
-            st = lib.sv_layer_norm_fwd(x2.data_ptr(), r2.data_ptr() if r2 is not None else None,
-                                       1 if x.dtype == torch.bfloat16 else 0, R, D, gamma.data_ptr(), beta.data_ptr(),
-                                       float(eps), float(p), int(seed), y.data_ptr(), s.data_ptr() if need_s else None,
-                                       stats[0].data_ptr(), stats[1].data_ptr(),
-                                       torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(lib, st, "sv_layer_norm_fwd")
+        _lib.call(_lib.gps(), "sv_layer_norm_fwd", x.device, x2.data_ptr(), _lib.ptr(r2), 1 if x.dtype == torch.bfloat16 else 0,
+                  R, D, gamma.data_ptr(), beta.data_ptr(), float(eps), float(p), int(seed), y.data_ptr(), _lib.ptr(s),
+                  stats[0].data_ptr(), stats[1].data_ptr())
         ctx.save_for_backward(s if need_s else x2, gamma, stats)
         ctx.meta = (float(p), int(seed), residual is not None, x.shape)
         ctx.params = (gamma, beta)
@@ -801,13 +764,9 @@ class _LayerNormFn(torch.autograd.Function):
         dg_t, db_t = (pg.grad, pb.grad) if direct else (dgb[0], dgb[1])
         lib = _lib.gps()
         scratch = torch.empty(lib.sv_layer_norm_scratch_floats(D), dtype=torch.float32, device=s.device)
-        with torch.cuda.device(s.device):
-            st = lib.sv_layer_norm_bwd_acc(g2.data_ptr(), s.data_ptr(), 1 if s.dtype == torch.bfloat16 else 0, R, D,
-                                           gamma.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), p, seed, ds.data_ptr(),
-                                           dx.data_ptr() if dx is not None else None, dg_t.data_ptr(), db_t.data_ptr(),
-                                           1 if direct else 0, scratch.data_ptr(),
-                                           torch.cuda.current_stream(s.device).cuda_stream)
-        _lib.check(lib, st, "sv_layer_norm_bwd_acc")
+        _lib.call(lib, "sv_layer_norm_bwd_acc", s.device, g2.data_ptr(), s.data_ptr(), 1 if s.dtype == torch.bfloat16 else 0, R,
+                  D, gamma.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), p, seed, ds.data_ptr(), _lib.ptr(dx),
+                  dg_t.data_ptr(), db_t.data_ptr(), 1 if direct else 0, scratch.data_ptr())
         d_x = (dx if dx is not None else ds).view(shape)
         return d_x, (ds.view(shape) if has_res else None), (None if direct else dgb[0]), (None if direct else dgb[1]), None, None, None
 
@@ -847,15 +806,13 @@ class _L2NormalizeFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, eps):
         from . import _lib
-        lib = _lib.gps()
         D = x.shape[-1]
         x2 = x.reshape(-1, D).contiguous()
         R = x2.shape[0]
         y = torch.empty_like(x2)
         norm = torch.empty(R, dtype=torch.float32, device=x.device)
-        st = lib.sv_l2norm_fwd(x2.data_ptr(), int(x2.dtype == torch.bfloat16), R, D, float(eps), y.data_ptr(), norm.data_ptr(),
-                               torch.cuda.current_stream(x.device).cuda_stream)
-        _lib.check(lib, st, "sv_l2norm_fwd")
+        _lib.call(_lib.gps(), "sv_l2norm_fwd", x.device, x2.data_ptr(), int(x2.dtype == torch.bfloat16), R, D, float(eps),
+                  y.data_ptr(), norm.data_ptr())
         ctx.save_for_backward(y, norm)
         ctx.eps, ctx.shape = float(eps), x.shape
         return y.view(x.shape)
@@ -863,14 +820,12 @@ class _L2NormalizeFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad):
         from . import _lib
-        lib = _lib.gps()
         y, norm = ctx.saved_tensors
         R, D = y.shape
         g2 = grad.reshape(R, D).to(y.dtype).contiguous()
         dx = torch.empty_like(y)
-        st = lib.sv_l2norm_bwd(g2.data_ptr(), y.data_ptr(), norm.data_ptr(), int(y.dtype == torch.bfloat16), R, D, ctx.eps,
-                               dx.data_ptr(), torch.cuda.current_stream(y.device).cuda_stream)
-        _lib.check(lib, st, "sv_l2norm_bwd")
+        _lib.call(_lib.gps(), "sv_l2norm_bwd", y.device, g2.data_ptr(), y.data_ptr(), norm.data_ptr(),
+                  int(y.dtype == torch.bfloat16), R, D, ctx.eps, dx.data_ptr())
         return dx.view(ctx.shape), None
 
 

@@ -12,10 +12,6 @@ import torch.nn.functional as F
 from . import _lib, native
 
 
-def _st(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def _round8(n):
     return (n + 7) // 8 * 8
 
@@ -29,13 +25,11 @@ class _GroupRowsFn(torch.autograd.Function):
         C = 0 if feat is None else feat.shape[-1]
         Cp = _round8(3 + C)
         X = torch.empty((B * np_ * ns, Cp), dtype=torch.bfloat16, device=xyz.device)
-        lib = _lib.gps()
         xyz, feat = xyz.contiguous(), (feat.contiguous() if feat is not None else None)
-        with torch.cuda.device(xyz.device):
-            st = lib.sv_pn_group_rows(xyz.data_ptr(), centre.contiguous().data_ptr() if centre is not None else None,
-                                      feat.data_ptr() if feat is not None else None, 1 if (feat is not None and feat.dtype == torch.bfloat16) else 0,
-                                      idx.data_ptr() if idx is not None else None, B, N, C, np_, ns, Cp, X.data_ptr(), _st(xyz))
-        _lib.check(lib, st, "sv_pn_group_rows")
+        centre = centre.contiguous() if centre is not None else None
+        _lib.call(_lib.gps(), "sv_pn_group_rows", xyz.device, xyz.data_ptr(), _lib.ptr(centre), _lib.ptr(feat),
+                  1 if (feat is not None and feat.dtype == torch.bfloat16) else 0, _lib.ptr(idx), B, N, C, np_, ns, Cp,
+                  X.data_ptr())
         ctx.save_for_backward(idx)
         ctx.meta = (B, N, C, np_, ns, Cp, None if feat is None else feat.dtype)
         return X
@@ -48,11 +42,8 @@ class _GroupRowsFn(torch.autograd.Function):
             return None, None, None, None, None, None
         dX = dX.contiguous()
         dfeat = torch.empty((B, N, C), dtype=torch.float32, device=dX.device)
-        lib = _lib.gps()
-        with torch.cuda.device(dX.device):
-            st = lib.sv_pn_group_rows_grad(dX.data_ptr(), idx.data_ptr() if idx is not None else None, B, N, C, np_, ns, Cp,
-                                           dfeat.data_ptr(), _st(dX))
-        _lib.check(lib, st, "sv_pn_group_rows_grad")
+        _lib.call(_lib.gps(), "sv_pn_group_rows_grad", dX.device, dX.data_ptr(), _lib.ptr(idx), B, N, C, np_, ns, Cp,
+                  dfeat.data_ptr())
         return None, None, dfeat.to(fdt), None, None, None
 
 
@@ -111,24 +102,19 @@ class StatExchange:
         assert C <= self.CAP
         lib = _lib.gps()
         scratch = torch.empty(lib.sv_pn_scratch_floats(C), dtype=torch.float32, device=y.device)
-        p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-        with torch.cuda.device(y.device):
-            st = lib.sv_pn_bn_sync_push(mode, p(y), p(dout), R, C, p(g32), p(b32), p(stats[0]) if stats is not None else None,
-                                        p(stats[1]) if stats is not None else None, scratch.data_ptr(), self.peer_bufs.data_ptr(),
-                                        self.CAP, self.done.data_ptr(), self.world, self.rank, self.epoch_dev.data_ptr(), _st(y))
-        _lib.check(lib, st, "sv_pn_bn_sync_push")
+        mean, rstd = (stats[0], stats[1]) if stats is not None else (None, None)
+        _lib.call(lib, "sv_pn_bn_sync_push", y.device, mode, y.data_ptr(), _lib.ptr(dout), R, C, _lib.ptr(g32), _lib.ptr(b32),
+                  _lib.ptr(mean), _lib.ptr(rstd), scratch.data_ptr(), self.peer_bufs.data_ptr(), self.CAP, self.done.data_ptr(),
+                  self.world, self.rank, self.epoch_dev.data_ptr())
 
     def finish_fwd(self, y, g32, b32, eps):
         """-> (relu(BN(y)) bf16, stats (3, C) f32: global mean, rstd, unbiased variance)."""
         R, C = y.shape
         stats = torch.empty((3, C), dtype=torch.float32, device=y.device)
         out = torch.empty_like(y)
-        lib = _lib.gps()
-        with torch.cuda.device(y.device):
-            st = lib.sv_pn_bn_sync_finish_fwd(y.data_ptr(), R, C, g32.data_ptr(), b32.data_ptr(), float(eps), stats[0].data_ptr(),
-                                              stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(), self.peer_bufs.data_ptr(),
-                                              self.CAP, self.world, self.rank, self.epoch_dev.data_ptr(), _st(y))
-        _lib.check(lib, st, "sv_pn_bn_sync_finish_fwd")
+        _lib.call(_lib.gps(), "sv_pn_bn_sync_finish_fwd", y.device, y.data_ptr(), R, C, g32.data_ptr(), b32.data_ptr(),
+                  float(eps), stats[0].data_ptr(), stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(),
+                  self.peer_bufs.data_ptr(), self.CAP, self.world, self.rank, self.epoch_dev.data_ptr())
         return out, stats
 
     def finish_bwd(self, y, dout, stats, g32, b32):
@@ -137,13 +123,9 @@ class StatExchange:
         dy = torch.empty_like(y)
         dgb = torch.empty((2, C), dtype=torch.float32, device=y.device)
         gsum = torch.empty(2 * C + 1, dtype=torch.float32, device=y.device)
-        lib = _lib.gps()
-        with torch.cuda.device(y.device):
-            st = lib.sv_pn_bn_sync_finish_bwd(y.data_ptr(), dout.data_ptr(), R, C, g32.data_ptr(), b32.data_ptr(), stats[0].data_ptr(),
-                                              stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(), 0,
-                                              gsum.data_ptr(), self.peer_bufs.data_ptr(), self.CAP, self.world, self.rank,
-                                              self.epoch_dev.data_ptr(), _st(y))
-        _lib.check(lib, st, "sv_pn_bn_sync_finish_bwd")
+        _lib.call(_lib.gps(), "sv_pn_bn_sync_finish_bwd", y.device, y.data_ptr(), dout.data_ptr(), R, C, g32.data_ptr(),
+                  b32.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(),
+                  0, gsum.data_ptr(), self.peer_bufs.data_ptr(), self.CAP, self.world, self.rank, self.epoch_dev.data_ptr())
         return dy, dgb
 
 
@@ -181,10 +163,8 @@ class _ConvBNReLUFn(torch.autograd.Function):
             out = torch.empty_like(y)
             lib = _lib.gps()
             scratch = torch.empty(lib.sv_pn_scratch_floats(Cout), dtype=torch.float32, device=X.device)
-            with torch.cuda.device(X.device):
-                st = lib.sv_pn_bn_relu_fwd(y.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), float(eps), stats[0].data_ptr(),
-                                           stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(), scratch.data_ptr(), _st(X))
-            _lib.check(lib, st, "sv_pn_bn_relu_fwd")
+            _lib.call(lib, "sv_pn_bn_relu_fwd", X.device, y.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), float(eps),
+                      stats[0].data_ptr(), stats[1].data_ptr(), stats[2].data_ptr(), out.data_ptr(), scratch.data_ptr())
         ctx.save_for_backward(X, wb, y, stats, g32, b32)
         ctx.cin, ctx.ex = Cin, ex
         ctx.mark_non_differentiable(stats)
@@ -203,11 +183,9 @@ class _ConvBNReLUFn(torch.autograd.Function):
             dgb = torch.empty((2, Cout), dtype=torch.float32, device=y.device)
             lib = _lib.gps()
             scratch = torch.empty(lib.sv_pn_scratch_floats(Cout), dtype=torch.float32, device=y.device)
-            with torch.cuda.device(y.device):
-                st = lib.sv_pn_bn_relu_bwd(y.data_ptr(), dout.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(), stats[0].data_ptr(),
-                                           stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(), 0,
-                                           scratch.data_ptr(), _st(y))
-            _lib.check(lib, st, "sv_pn_bn_relu_bwd")
+            _lib.call(lib, "sv_pn_bn_relu_bwd", y.device, y.data_ptr(), dout.data_ptr(), R, Cout, g32.data_ptr(), b32.data_ptr(),
+                      stats[0].data_ptr(), stats[1].data_ptr(), dy.data_ptr(), dgb[0].data_ptr(), dgb[1].data_ptr(), 0,
+                      scratch.data_ptr())
         dX, dw = _ConvBNReLUFn.conv_bwd(X, wb, dy, ctx.cin, ctx.needs_input_grad[0])
         return dX, dw, dgb[0], dgb[1], None, None
 
@@ -219,10 +197,7 @@ class _RowGroupMaxFn(torch.autograd.Function):
         G = R // ns
         out = torch.empty((G, C), dtype=torch.bfloat16, device=x.device)
         arg = torch.empty((G, C), dtype=torch.uint8, device=x.device)
-        lib = _lib.gps()
-        with torch.cuda.device(x.device):
-            st = lib.sv_pn_rowgroup_max(x.data_ptr(), G, ns, C, out.data_ptr(), arg.data_ptr(), _st(x))
-        _lib.check(lib, st, "sv_pn_rowgroup_max")
+        _lib.call(_lib.gps(), "sv_pn_rowgroup_max", x.device, x.data_ptr(), G, ns, C, out.data_ptr(), arg.data_ptr())
         ctx.save_for_backward(arg)
         ctx.ns = ns
         return out
@@ -233,10 +208,7 @@ class _RowGroupMaxFn(torch.autograd.Function):
         G, C = arg.shape
         g = g.contiguous().to(torch.bfloat16)
         gx = torch.empty((G * ctx.ns, C), dtype=torch.bfloat16, device=g.device)
-        lib = _lib.gps()
-        with torch.cuda.device(g.device):
-            st = lib.sv_pn_rowgroup_max_grad(g.data_ptr(), arg.data_ptr(), G, ctx.ns, C, gx.data_ptr(), _st(g))
-        _lib.check(lib, st, "sv_pn_rowgroup_max_grad")
+        _lib.call(_lib.gps(), "sv_pn_rowgroup_max_grad", g.device, g.data_ptr(), arg.data_ptr(), G, ctx.ns, C, gx.data_ptr())
         return gx, None
 
 

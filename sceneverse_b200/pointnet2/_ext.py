@@ -30,24 +30,13 @@ def _cuda_only(t, *others):
             raise RuntimeError("tensors must be on the same device")
 
 
-def _stream(t):
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
-def _run(fn_name, dev_tensor, *args):
-    lib = _lib.pointops()
-    with torch.cuda.device(dev_tensor.device):
-        st = getattr(lib, fn_name)(*args, _stream(dev_tensor))
-    _lib.check(lib, st, fn_name)
-
-
 def furthest_point_sampling(points, nsamples):
     """sampling.cpp:66-87.  (B,N,3) f32 -> (B,nsamples) i32."""
     _check(points, "points", torch.float32)
     _cuda_only(points)
     B, N, _ = points.shape
     out = torch.empty((B, nsamples), dtype=torch.int32, device=points.device)
-    _run("sv_fps_f32", points, points.data_ptr(), B, N, int(nsamples), out.data_ptr(), None)
+    _lib.call(_lib.pointops(), "sv_fps_f32", points.device, points.data_ptr(), B, N, int(nsamples), out.data_ptr(), None)
     return out
 
 
@@ -59,7 +48,8 @@ def gather_points(points, idx):
     B, C, N = points.shape
     M = idx.shape[1]
     out = torch.empty((B, C, M), dtype=torch.float32, device=points.device)
-    _run("sv_gather_points_f32", points, points.data_ptr(), idx.data_ptr(), B, C, N, M, out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_gather_points_f32", points.device, points.data_ptr(), idx.data_ptr(), B, C, N, M,
+              out.data_ptr())
     return out
 
 
@@ -70,7 +60,8 @@ def gather_points_grad(grad_out, idx, n):
     _cuda_only(grad_out, idx)
     B, C, M = grad_out.shape
     out = torch.empty((B, C, int(n)), dtype=torch.float32, device=grad_out.device)
-    _run("sv_gather_points_grad_f32", grad_out, grad_out.data_ptr(), idx.data_ptr(), B, C, int(n), M, out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_gather_points_grad_f32", grad_out.device, grad_out.data_ptr(), idx.data_ptr(), B, C, int(n),
+              M, out.data_ptr())
     return out
 
 
@@ -82,8 +73,8 @@ def ball_query(new_xyz, xyz, radius, nsample):
     B, M, _ = new_xyz.shape
     N = xyz.shape[1]
     out = torch.empty((B, M, int(nsample)), dtype=torch.int32, device=new_xyz.device)
-    _run("sv_ball_query_f32", new_xyz, new_xyz.data_ptr(), xyz.data_ptr(), B, N, M, float(radius), int(nsample),
-         out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_ball_query_f32", new_xyz.device, new_xyz.data_ptr(), xyz.data_ptr(), B, N, M, float(radius),
+              int(nsample), out.data_ptr())
     return out
 
 
@@ -95,7 +86,8 @@ def group_points(points, idx):
     B, C, N = points.shape
     _, NP, NS = idx.shape
     out = torch.empty((B, C, NP, NS), dtype=torch.float32, device=points.device)
-    _run("sv_group_points_f32", points, points.data_ptr(), idx.data_ptr(), B, C, N, NP, NS, out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_group_points_f32", points.device, points.data_ptr(), idx.data_ptr(), B, C, N, NP, NS,
+              out.data_ptr())
     return out
 
 
@@ -106,8 +98,8 @@ def group_points_grad(grad_out, idx, n):
     _cuda_only(grad_out, idx)
     B, C, NP, NS = grad_out.shape
     out = torch.empty((B, C, int(n)), dtype=torch.float32, device=grad_out.device)
-    _run("sv_group_points_grad_f32", grad_out, grad_out.data_ptr(), idx.data_ptr(), B, C, int(n), NP, NS,
-         out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_group_points_grad_f32", grad_out.device, grad_out.data_ptr(), idx.data_ptr(), B, C, int(n),
+              NP, NS, out.data_ptr())
     return out
 
 
@@ -120,7 +112,8 @@ def three_nn(unknowns, knows):
     m = knows.shape[1]
     idx = torch.empty((B, n, 3), dtype=torch.int32, device=unknowns.device)
     dist2 = torch.empty((B, n, 3), dtype=torch.float32, device=unknowns.device)
-    _run("sv_three_nn_f32", unknowns, unknowns.data_ptr(), knows.data_ptr(), B, n, m, dist2.data_ptr(), idx.data_ptr())
+    _lib.call(_lib.pointops(), "sv_three_nn_f32", unknowns.device, unknowns.data_ptr(), knows.data_ptr(), B, n, m,
+              dist2.data_ptr(), idx.data_ptr())
     return [dist2, idx]
 
 
@@ -133,8 +126,8 @@ def three_interpolate(points, idx, weight):
     B, c, m = points.shape
     n = idx.shape[1]
     out = torch.empty((B, c, n), dtype=torch.float32, device=points.device)
-    _run("sv_three_interpolate_f32", points, points.data_ptr(), idx.data_ptr(), weight.data_ptr(), B, c, m, n,
-         out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_three_interpolate_f32", points.device, points.data_ptr(), idx.data_ptr(), weight.data_ptr(),
+              B, c, m, n, out.data_ptr())
     return out
 
 
@@ -146,8 +139,8 @@ def three_interpolate_grad(grad_out, idx, weight, m):
     _cuda_only(grad_out, idx, weight)
     B, c, n = grad_out.shape
     out = torch.empty((B, c, int(m)), dtype=torch.float32, device=grad_out.device)
-    _run("sv_three_interpolate_grad_f32", grad_out, grad_out.data_ptr(), idx.data_ptr(), weight.data_ptr(), B, c, n,
-         int(m), out.data_ptr())
+    _lib.call(_lib.pointops(), "sv_three_interpolate_grad_f32", grad_out.device, grad_out.data_ptr(), idx.data_ptr(),
+              weight.data_ptr(), B, c, n, int(m), out.data_ptr())
     return out
 
 
@@ -162,11 +155,11 @@ def fps_ballquery(xyz, npoint, radius, nsample):
     new_xyz = torch.empty((B, npoint, 3), dtype=torch.float32, device=xyz.device)
     ball_idx = torch.empty((B, npoint, nsample), dtype=torch.int32, device=xyz.device)
     if 32 <= N <= 1024:
-        _run("sv_sa_sample_f32", xyz, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
-             fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr(), 0, 0.0, 0, None, None, None)
+        _lib.call(_lib.pointops(), "sv_sa_sample_f32", xyz.device, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
+                  fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr(), 0, 0.0, 0, None, None, None)
     else:
-        _run("sv_fps_ballquery_f32", xyz, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
-             fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr())
+        _lib.call(_lib.pointops(), "sv_fps_ballquery_f32", xyz.device, xyz.data_ptr(), B, N, int(npoint), float(radius),
+                  int(nsample), fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr())
     return fps_idx, new_xyz, ball_idx
 
 
@@ -179,8 +172,8 @@ def fps_ballquery_scan(xyz, npoint, radius, nsample):
     fps_idx = torch.empty((B, npoint), dtype=torch.int32, device=xyz.device)
     new_xyz = torch.empty((B, npoint, 3), dtype=torch.float32, device=xyz.device)
     ball_idx = torch.empty((B, npoint, nsample), dtype=torch.int32, device=xyz.device)
-    _run("sv_fps_ballquery_f32", xyz, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
-         fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr())
+    _lib.call(_lib.pointops(), "sv_fps_ballquery_f32", xyz.device, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
+              fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr())
     return fps_idx, new_xyz, ball_idx
 
 
@@ -197,7 +190,7 @@ def sa_sample2(xyz, npoint, radius, nsample, npoint2, radius2, nsample2):
     fps_idx2 = torch.empty((B, npoint2), dtype=torch.int32, device=dev)
     new_xyz2 = torch.empty((B, npoint2, 3), dtype=torch.float32, device=dev)
     ball_idx2 = torch.empty((B, npoint2, nsample2), dtype=torch.int32, device=dev)
-    _run("sv_sa_sample_f32", xyz, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
-         fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr(), int(npoint2), float(radius2), int(nsample2),
-         fps_idx2.data_ptr(), new_xyz2.data_ptr(), ball_idx2.data_ptr())
+    _lib.call(_lib.pointops(), "sv_sa_sample_f32", xyz.device, xyz.data_ptr(), B, N, int(npoint), float(radius), int(nsample),
+              fps_idx.data_ptr(), new_xyz.data_ptr(), ball_idx.data_ptr(), int(npoint2), float(radius2), int(nsample2),
+              fps_idx2.data_ptr(), new_xyz2.data_ptr(), ball_idx2.data_ptr())
     return fps_idx, new_xyz, ball_idx, fps_idx2, new_xyz2, ball_idx2

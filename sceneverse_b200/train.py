@@ -466,16 +466,12 @@ class FlatState(FlatGrads):
     def optimizer_step(self):
         """clip (max_norm) + AdamW + shadow refresh; the step counter lives on the device (CUDA-graph replay safe)."""
         from . import _lib
-        lib = _lib.gps()
         self.step_t.add_(1)
-        with torch.cuda.device(self.flat.device):
-            st = lib.sv_adamw_flat(self.flat_p.data_ptr(), self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(),
-                                   self.flat.data_ptr(), self.shadow.data_ptr(), self.n, self.segments.data_ptr(), self.nseg,
-                                   float(self.max_norm) if self.max_norm is not None else 0.0, self.lr_factor.data_ptr(),
-                                   self.step_t.data_ptr(), 1.0, float(self.betas[0]), float(self.betas[1]), float(self.eps),
-                                   self.scratch.data_ptr(), self.grad_norm_t.data_ptr(),
-                                   torch.cuda.current_stream(self.flat.device).cuda_stream)
-        _lib.check(lib, st, "sv_adamw_flat")
+        _lib.call(_lib.gps(), "sv_adamw_flat", self.flat.device, self.flat_p.data_ptr(), self.exp_avg.data_ptr(),
+                  self.exp_avg_sq.data_ptr(), self.flat.data_ptr(), self.shadow.data_ptr(), self.n, self.segments.data_ptr(),
+                  self.nseg, float(self.max_norm) if self.max_norm is not None else 0.0, self.lr_factor.data_ptr(),
+                  self.step_t.data_ptr(), 1.0, float(self.betas[0]), float(self.betas[1]), float(self.eps),
+                  self.scratch.data_ptr(), self.grad_norm_t.data_ptr())
 
 
 def register_packs(module, flat):

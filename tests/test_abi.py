@@ -85,3 +85,34 @@ def test_gps_argument_validation_without_gpu(built):
     assert lib.sv_attention_fwd_dropout_bf16(fake, 8, 8, fake, 8, 8, fake, 8, 8, fake, 8, 8, None, None, 0, None, 1, 12, 4,
                                              400, 0.125, None, 0.0, 0, None) == 1                                      # Lk > 384
     assert lib.sv_layer_norm_scratch_floats(768) > 0 and lib.sv_colsum_scratch_floats(768) > 0
+
+
+def test_argtypes_bound_from_headers(built):
+    """After loading, every prototype of both headers has argtypes, one per parameter the header declares."""
+    from sceneverse_b200 import _lib
+    for header, lib in (("svpointops.h", _lib.pointops()), ("svgps.h", _lib.gps())):
+        src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", header)).read(), flags=re.S)
+        protos = re.findall(r"\b(sv\w*)\s*\(([^()]*)\)\s*;", src)
+        assert len(protos) > 10, header
+        for name, params in protos:
+            n_params = 0 if params.strip() == "void" else params.count(",") + 1
+            argtypes = getattr(lib, name).argtypes
+            assert argtypes is not None and len(argtypes) == n_params, (header, name, argtypes)
+
+
+def test_header_types_pinned(built):
+    from sceneverse_b200 import _lib
+    pointops, gps = _lib.pointops(), _lib.gps()
+    assert pointops.sv_scene_prep_aug_f32.argtypes[5] is ctypes.POINTER(_lib.AugParams)
+    fwd = gps.sv_attention_fwd_dropout_bf16.argtypes
+    assert fwd[22] is ctypes.c_float and fwd[23] is ctypes.c_ulonglong   # dropout_p, seed
+    assert pointops.sv_status_string.restype is ctypes.c_char_p
+    assert pointops.sv_launch_count.restype is ctypes.c_ulonglong
+    assert gps.svgps_launch_count.restype is ctypes.c_ulonglong
+
+
+@pytest.mark.parametrize("proto", ["int sv_x(size_t n, void *stream);", "size_t sv_x(int n);"])
+def test_unknown_header_type_raises(proto):
+    from sceneverse_b200 import _lib
+    with pytest.raises(_lib.NativeLibraryError, match="sv_x"):
+        _lib.parse_prototypes(proto)
