@@ -67,6 +67,7 @@ struct GemmArgs {
   int red_out;              // WGRAD: accumulate into out with atomic adds instead of storing
   float *bias_grad;         // WGRAD: [M] += row sums of A (the bias gradient), or null
   int n_tma;                // OUT_TMA: columns [0, n_tma) go out by TMA, the rest of [0, N) per element (see run_gemm)
+  int aux_tma;              // DGRAD with OUT_TMA and bf16 out: aux is loaded by TMA through mapO2 (see run_gemm)
 };
 
 // Phi(x) = 0.5 (1 + erf(x / sqrt 2)) and e = exp(-x^2 / 2) with two MUFU ops: erf by Abramowitz-Stegun 7.1.26
@@ -111,12 +112,13 @@ template <int BN, int OUT_TMA>
 struct GemmCfg {
   static constexpr int A_STAGE = BM * BK * 2, B_STAGE = BN * BK * 2;
   static constexpr int OUT = OUT_TMA ? 2 * OUT_RING : 0;   // the output rings of the two consumer warpgroups
+  static constexpr int BARS = 2 * 8 + 4;                   // full / empty of at most 8 stages, 2 x 2 aux-box barriers
   // OUT_TMA: operand stages fill what is left after the output rings, 1 KB alignment slack, the 1 KB tile of ones (WGRAD
-  // bias-gradient operand) and the barriers of at most 8 stages.  The per-element kernels keep their 200 KB operand budget.
+  // bias-gradient operand) and the barriers.  The per-element kernels keep their 200 KB operand budget.
   static constexpr int STAGES_RAW =
-      OUT_TMA ? (SMEM_OPTIN - OUT - 1024 - 1024 - 2 * 8 * 8) / (A_STAGE + B_STAGE) : (200 * 1024) / (A_STAGE + B_STAGE);
+      OUT_TMA ? (SMEM_OPTIN - OUT - 1024 - 1024 - BARS * 8) / (A_STAGE + B_STAGE) : (200 * 1024) / (A_STAGE + B_STAGE);
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + OUT + 1024 + 1024 + 2 * STAGES * 8;
+  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + OUT + 1024 + 1024 + BARS * 8;
   static_assert(SMEM <= SMEM_OPTIN, "gemm_kernel shared memory exceeds the opt-in limit");
 };
 
@@ -150,7 +152,8 @@ __device__ __forceinline__ void mma(float (&d)[BN / 2], uint64_t da, uint64_t db
 }
 
 // OUT_TMA = 1: the epilogue stages out (and out2) in shared memory and writes them by TMA store (WGRAD: TMA reduce-add)
-// through mapO / mapO2; 0: per-element stores (the maps are unused)
+// through mapO / mapO2; 0: per-element stores (the maps are unused).  With g.aux_tma, mapO2 is the DGRAD saved activation,
+// whose boxes are loaded into the ring slots the same columns go out through.
 template <int BN, int EPI, int TA, int TB, int OUT_TMA>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
@@ -165,6 +168,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   uint8_t *sOnes = sOut + Cfg::OUT;                            // [8][64] bf16 ones (1 KB), WGRAD bias-gradient operand
   uint64_t *full = reinterpret_cast<uint64_t *>(sOnes + 1024);
   uint64_t *empty = full + STAGES;
+  uint64_t *auxb = empty + STAGES;                             // [2 consumer warpgroups][2 ring slots]: aux box landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
@@ -179,6 +183,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       mbar_init(full + s, 1);
       mbar_init(empty + s, 2);   // one arrival per consumer warpgroup
     }
+    for (int i = 0; i < 4; ++i) mbar_init(auxb + i, 1);
     mbar_fence_init();
   }
   if (EPI == EPI_WGRAD) {
@@ -240,7 +245,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   const bool f32_out = EPI == EPI_WGRAD || g.out_f32;
   const int box_j = f32_out ? 4 : 8;
   const uint32_t ring = smem_u32(sOut) + (uint32_t)c * OUT_RING;
-  // this lane's byte offsets inside a box: stmatrix row addresses (bf16), or its two fp32 columns of row r_lo - 64 c
+  // DGRAD with a TMA-loadable saved activation: box k's aux tile is loaded into the ring slot box k is staged in, all of a
+  // tile's boxes (at most two: the ring) before its main loop.  Not at BN = 192: three boxes would not fit the ring, and with
+  // both aux paths in one kernel its epilogue spills, so it keeps the per-element loads.
+  const bool aux_tma = tma_out && EPI == EPI_DGRAD && BN <= 128 && g.aux_tma && !(g.dbg & 1);
+  uint64_t *my_auxb = auxb + 2 * c;
+  uint32_t aux_ph = 0;   // bit k: parity of ring slot k's next aux load
+  // this lane's byte offsets inside a box: stmatrix / ldmatrix row addresses (bf16), or its two fp32 columns of row r_lo - 64 c
   const uint32_t sm_row = (uint32_t)(w * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * 128u, sm_x = lane & 7, sm_j = lane >> 4;
   const uint32_t f_row = (uint32_t)(w * 16 + (lane >> 2)) * 128u, f_hi = (lane >> 1) & 1, f_x = lane >> 2, f_lo = (lane & 1) * 8u;
   uint32_t nbox = 0;
@@ -256,6 +267,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     const int m0 = tmi * BM, n0 = tni * BN;
     const int ks0 = sp * kps, ks1 = min(k_steps, ks0 + kps);
     const bool bias_tile = with_bias_grad && n0 == 0;
+    if (aux_tma && m0 + 64 * c < g.M) {
+      // the aux boxes land during the main loop; the ring is free once every thread has read the last tile's boxes (the
+      // per-element tail) and the last stores have read them
+      wg_sync(1 + c);
+      if (t == 0) {
+        bulk_wait_read<0>();
+        for (int b = 0; b < BN / 64 && n0 + 64 * b < g.N; ++b) {
+          const uint32_t slot = (nbox + (uint32_t)b) & 1u;
+          mbar_expect_tx(my_auxb + slot, OUT_BOX);
+          tma_load_2d(ring + slot * OUT_BOX, &mapO2, n0 + 64 * b, m0 + 64 * c, my_auxb + slot);
+        }
+      }
+    }
     uint32_t prev = 0;
     for (int ks = ks0; ks < ks1; ++ks, ++nks) {
       long long c0 = g.prof ? clock64() : 0;
@@ -280,7 +304,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     fence_regs(acc);
     if (EPI == EPI_WGRAD) fence_regs(accb);
     if (t == 0) mbar_arrive(empty + prev);
-    if (g.dbg & 1) continue;
+    if ((g.dbg & 1) || m0 + 64 * c >= g.M) continue;   // no rows of this warpgroup to write
 
     // ---- epilogue: element (row r_lo + 8 h, column 8 j + cq + e) is acc[4 j + 2 h + e] ----
     uint32_t rk[2] = {0u, 0u};
@@ -298,13 +322,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       // boxes that start at or past N are not staged, so the box holding column N - 1 is the last one of the tile
       if (tma_out && n0 + 8 * (jc - jc % box_j) >= g.N) break;
       if (tma_out && jc % box_j == 0) {
-        // the slot(s) this box is staged in must have been read out by the TMA store that last used them
-        if (t == 0) {
-          if (g.out2 != nullptr) bulk_wait_read<0>();
-          else bulk_wait_read<1>();
+        if (aux_tma) {
+          // this box's aux tile has landed in its slot (the slot was free when it was loaded)
+          const uint32_t slot = nbox & 1u;
+          mbar_wait(my_auxb + slot, (aux_ph >> slot) & 1u);
+          aux_ph ^= 1u << slot;
+        } else {
+          // the slot(s) this box is staged in must have been read out by the TMA store that last used them
+          if (t == 0) {
+            if (g.out2 != nullptr) bulk_wait_read<0>();
+            else bulk_wait_read<1>();
+          }
+          wg_sync(1 + c);
         }
-        wg_sync(1 + c);
       }
+      const uint32_t box = ring + (g.out2 != nullptr ? (uint32_t)OUT_BOX : (nbox & 1u) * OUT_BOX);
       float bv[2 * JB], xv[2 * JB][2];
       uint32_t pre[2 * JB];   // tma_out with out2: the packed bf16 pre-activation of (jj, h)
       if (EPI == EPI_FWD && g.bias != nullptr) {
@@ -316,15 +348,30 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         }
       }
       if (EPI == EPI_DGRAD && g.act != 0) {
-        const __nv_bfloat16 *ax = reinterpret_cast<const __nv_bfloat16 *>(g.aux);
+        if (aux_tma) {
+          // the aux box has the layout the output box is written in: ldmatrix returns the accumulator's fragments
 #pragma unroll
-        for (int jj = 0; jj < JB; ++jj) {
-          const int col = n0 + 8 * (jc + jj) + cq;
+          for (int jj = 0; jj < JB; jj += 2) {
+            const uint32_t a = sm_row + (((((uint32_t)(jc + jj) + sm_j) & 7u) ^ sm_x) << 4);
+            uint32_t r[4];
+            ldmatrix_x4(box + a, r[0], r[1], r[2], r[3]);
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const size_t r = (size_t)min(m0 + r_lo + 8 * h, g.M - 1) * g.ld_aux;
-            xv[2 * jj + h][0] = __bfloat162float(ax[r + min(col, g.N - 1)]);
-            xv[2 * jj + h][1] = __bfloat162float(ax[r + min(col + 1, g.N - 1)]);
+            for (int i = 0; i < 4; ++i) {   // r[i] = (h i % 2, column group jj + i / 2)
+              xv[2 * jj + i][0] = __uint_as_float(r[i] << 16);
+              xv[2 * jj + i][1] = __uint_as_float(r[i] & 0xFFFF0000u);
+            }
+          }
+        } else {
+          const __nv_bfloat16 *ax = reinterpret_cast<const __nv_bfloat16 *>(g.aux);
+#pragma unroll
+          for (int jj = 0; jj < JB; ++jj) {
+            const int col = n0 + 8 * (jc + jj) + cq;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const size_t r = (size_t)min(m0 + r_lo + 8 * h, g.M - 1) * g.ld_aux;
+              xv[2 * jj + h][0] = __bfloat162float(ax[r + min(col, g.N - 1)]);
+              xv[2 * jj + h][1] = __bfloat162float(ax[r + min(col + 1, g.N - 1)]);
+            }
           }
         }
       }
@@ -438,7 +485,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         }
       }
       if (tma_out) {
-        const uint32_t box = ring + (g.out2 != nullptr ? (uint32_t)OUT_BOX : (nbox & 1u) * OUT_BOX);
         if (f32_out) {
 #pragma unroll
           for (int jj = 0; jj < JB; ++jj) {
@@ -585,16 +631,16 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap 
   return sv::after_launch();
 }
 
-// Tile selection: one 128-row tile costs max(math, operand traffic) per K step — 4 BN clk of wgmma at ~2 K bf16 FMA/clk/SM
-// against (16 KB of A + 128 B x BN of B) through TMA at ~100 B/clk — and the persistent grid runs ceil(tiles / SMs)
-// waves of it.
-float tile_cost(int bn) {
-  const float math = 4.0f * bn;
-  const float mem = (16384.f + 128.f * bn) / 100.f;
-  return math > mem ? math : mem;
+// Tile selection: the persistent grid runs ceil(tiles / SMs) waves of 128 x BN tiles, and one tile costs BN times a relative
+// cost per output column measured for each width and direction (scripts/time_gemm_shapes.py at every forced width on the GPS
+// step's shapes, one H100 80GB HBM3 at 700 W, DESIGN.md §4.1), relative to the 192-wide tile.  The 64-wide tiles re-load the
+// 128-row A panel for every 64 columns; the weight gradient's 128-wide tiles leave less of their reduce-add epilogue exposed.
+float tile_cost(int epi, int bn) {
+  static const float rel[3][3] = {{1.18f, 1.02f, 1.0f}, {1.02f, 1.0f, 1.0f}, {1.52f, 0.76f, 1.0f}};   // [epi][64, 128, 192]
+  return rel[epi][bn / 64 - 1] * (float)bn;
 }
 
-int pick_tile(int M, int N, int sms, bool wgrad) {
+int pick_tile(int M, int N, int sms, int epi) {
   const int cand[3] = {192, 128, 64};
   float best_cost = 1e30f;
   int best = 64;
@@ -603,9 +649,7 @@ int pick_tile(int M, int N, int sms, bool wgrad) {
     const int bn = cand[i];
     if (bn > 64 && bn - 64 >= ((N + 63) / 64) * 64) continue;          // wider than the problem by a whole 64-column slab
     const int tiles = tm * ((N + bn - 1) / bn);
-    // a weight gradient fills the machine through split-K, so only the per-area cost of the tile matters there
-    const float waves = wgrad ? (float)tiles / sms : (float)((tiles + sms - 1) / sms);
-    const float cost = waves * tile_cost(bn);
+    const float cost = (float)((tiles + sms - 1) / sms) * tile_cost(epi, bn);
     if (cost < best_cost * 0.999f) {
       best_cost = cost;
       best = bn;
@@ -647,7 +691,7 @@ int run_gemm(int epi, const void *A, int lda, int a_t, const void *B, int ldb, i
   g.n_fast = (long long)N <= (long long)M ? 1 : 0;
   g.dbg = g_gemm_dbg;
   g.prof = g_gemm_prof;
-  int bn = g_force_bn == 1 ? 64 : g_force_bn == 2 ? 128 : g_force_bn == 4 ? 192 : pick_tile(M, N, sms, epi == EPI_WGRAD);
+  int bn = g_force_bn == 1 ? 64 : g_force_bn == 2 ? 128 : g_force_bn == 4 ? 192 : pick_tile(M, N, sms, epi);
   g.splits = 1;
   if (epi == EPI_WGRAD && g.red_out) {
     // split-K: the output of a weight gradient is small (a few dozen tiles), the contraction runs over every token
@@ -685,6 +729,14 @@ int run_gemm(int epi, const void *A, int lda, int a_t, const void *B, int ldb, i
     if (rc) return rc;
     if (g.out2 != nullptr) {
       rc = make_out_map(&mo2, g.out2, M, g.n_tma, g.ldo, false);
+      if (rc) return rc;
+    }
+    // A dgrad's saved activation is loaded by TMA into the bf16 output box its columns go out through, when its rows take
+    // 16-byte-aligned boxes; loads zero-fill past [M, N], so its map spans all N columns.  Other pitches keep the loads per
+    // element.
+    g.aux_tma = epi == EPI_DGRAD && g.act != 0 && esz == 2 && al16(g.aux) && g.ld_aux >= N && ((size_t)g.ld_aux * 2) % 16 == 0;
+    if (g.aux_tma) {
+      rc = make_out_map(&mo2, const_cast<void *>(g.aux), M, N, g.ld_aux, false);
       if (rc) return rc;
     }
   }

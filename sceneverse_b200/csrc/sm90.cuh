@@ -80,6 +80,14 @@ __device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t
                : "memory");
 }
 
+// four 8x8 b16 matrices <- shared: the inverse of stmatrix_x4 (same addresses, same register layout)
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr)
+               : "memory");
+}
+
 // ---- wgmma descriptors ----------------------------------------------------------------------------
 // shared-memory matrix descriptor, SWIZZLE_128B (layout type 1 in bits [62,64)): [0,14) start >> 4 | [16,30) leading
 // byte offset >> 4 | [32,46) stride byte offset >> 4.  The stride byte offset is the distance between 8-row (K-major) or
