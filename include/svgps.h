@@ -284,7 +284,7 @@ int sv_normalize_allgather_dev_f32(const float *a, const float *b, int n, int D,
  * vector of sv_eval_counters_size(kind) doubles; the kernels ADD one batch into it (atomics, CUDA-graph replay safe).  Counts
  * are integers held exactly in float64.  Logits are bf16 (is_bf16 != 0) or f32 rows with a row stride in elements (padded
  * vocabularies are read in place).  valid: (B,) bytes or NULL (all valid); an item with valid 0 counts nothing. */
-enum { SV_EVAL_GROUNDING = 0, SV_EVAL_OBJ_CLS = 1, SV_EVAL_ANSWERS = 2 };
+enum { SV_EVAL_GROUNDING = 0, SV_EVAL_OBJ_CLS = 1, SV_EVAL_ANSWERS = 2, SV_EVAL_PRETRAIN = 3 };
 /* ScanReferEval / ReferIt3DEval: items; is_multiple / is_hard / is_view_dependent items; og_pred == tgt_object_id (all, hard,
  * view-dependent); IoU-25 / IoU-50 flag at og_pred (all, multiple); txt_acc; then up to three (hits, masked objects) pairs of
  * sv_eval_obj_cls at SV_EVG_OBJ. */
@@ -303,6 +303,18 @@ enum {
   SV_EVA_OBJ_COUNT = 16, SV_EVA_SNAPSHOT = 17, SV_EVA_Q_ANS1 = 34, SV_EVA_Q_ANS10 = 35, SV_EVA_Q_OBJ = 36, SV_EVA_Q_TYPE = 37,
   SV_EVA_Q_TYPE_COUNT = 43, SV_EVA_SIZE = 49
 };
+/* PretrainEval: the grounding words SV_EVG_ITEMS..SV_EVG_TXT_ACC at SV_EVP_OG (of them only og_acc is reported); items;
+ * masked-LM hits and labelled tokens; then, for each object logits tensor present in the order post, raw, pre (the
+ * SV_EVP_HAS_* bits), six words: (hits, rows) over obj_masks, obj_masks & obj_sem_masks, obj_masks & !obj_sem_masks.  Then
+ * a snapshot of those SV_EVP_SNAPSHOT integers at the end of the previous batch, and the float64 sums of per-batch metric x
+ * items at SV_EVP_Q + SV_EVP_Q_*, in the reference's eval_dict order. */
+enum {
+  SV_EVP_OG = 0, SV_EVP_ITEMS = SV_EVG_OBJ, SV_EVP_LM_HIT, SV_EVP_LM_COUNT, SV_EVP_OBJ, SV_EVP_SNAPSHOT = SV_EVP_OBJ + 18,
+  SV_EVP_Q = 2 * SV_EVP_SNAPSHOT, SV_EVP_SIZE = SV_EVP_Q + 10,
+  SV_EVP_Q_TARGET = 0, SV_EVP_Q_OG, SV_EVP_Q_LM, SV_EVP_Q_POST, SV_EVP_Q_PRE, SV_EVP_Q_RAW, SV_EVP_Q_PRE_UNMASK,
+  SV_EVP_Q_PRE_MASK, SV_EVP_Q_POST_UNMASK, SV_EVP_Q_POST_MASK,
+  SV_EVP_HAS_OG = 1, SV_EVP_HAS_POST = 2, SV_EVP_HAS_RAW = 4, SV_EVP_HAS_PRE = 8
+};
 int sv_eval_counters_size(int kind);
 /* og_pred = argmax of og3d_logits (B, O) (torch's rule: first maximum, NaN above everything), element (b, o) at
  * b * og_row_stride + o * og_col_stride (the grounding head writes it as column 0 of padded rows).  tgt_object_id (B) int64.
@@ -315,10 +327,12 @@ int sv_eval_grounding(const void *og3d_logits, int og_bf16, long long og_row_str
                       const unsigned char *is_view_dependent, const unsigned char *valid, double *counters, void *stream);
 /* Up to three (B, O, C) logits tensors (host arrays of device pointers / dtypes / strides in elements): for tensor t,
  * counters[2t] += #{masked objects whose argmax over C equals obj_labels}, counters[2t + 1] += #{masked objects}.
- * obj_labels (B, O) int64, obj_masks (B, O) bytes. */
+ * obj_labels (B, O) int64, obj_masks (B, O) bytes.  split_mask (B, O) bytes or NULL: tensor t then adds into
+ * counters[6t .. 6t + 5] the (hits, masked objects) pairs over obj_masks, obj_masks & split_mask, obj_masks & !split_mask. */
 int sv_eval_obj_cls(int n_logits, const void *const *logits, const int *is_bf16, const long long *row_stride,
                     const long long *item_stride, int B, int O, int C, const long long *obj_labels,
-                    const unsigned char *obj_masks, const unsigned char *valid, double *counters, void *stream);
+                    const unsigned char *obj_masks, const unsigned char *split_mask, const unsigned char *valid,
+                    double *counters, void *stream);
 /* answer_scores (B, A) rows; answer_label (B, A) int64 multi-hot (a 1 marks a correct answer).  Top-1 hit: the argmax is
  * labelled 1.  Top-10 hit: a labelled answer ranks among the first 10 (scores descending, NaN first, ties: lower index first).
  * sqa_type (B) int64 in 0..5 or NULL.  Adds into the SV_EVA_* words. */
@@ -326,6 +340,20 @@ int sv_eval_answers(const void *answer_scores, int is_bf16, long long row_stride
                     const long long *sqa_type, const unsigned char *valid, double *counters, void *stream);
 /* SQA3DEval.update's float64 bookkeeping for the batch just added (after sv_eval_answers and sv_eval_obj_cls of that batch). */
 int sv_eval_sqa3d_batch(double *counters, void *stream);
+/* Masked-LM accuracy: logits (R, V) rows (row_stride >= V elements; a padded vocabulary is read in place, its pad columns
+ * never), R = B * L token rows, masked_lm_labels (R) int64 with -1 = not labelled.  counters[SV_EVP_LM_HIT] += #{labelled rows
+ * whose argmax equals the label}, counters[SV_EVP_LM_COUNT] += #{labelled rows}, counters[SV_EVP_ITEMS] += #{valid items};
+ * row r belongs to item r / L. */
+int sv_eval_lm_acc(const void *logits, int is_bf16, long long row_stride, long long R, int V, int L,
+                   const long long *masked_lm_labels, const unsigned char *valid, double *counters, void *stream);
+/* PretrainEval.update's float64 bookkeeping for the batch just added; present = the SV_EVP_HAS_* bits of that batch. */
+int sv_eval_pretrain_batch(double *counters, int present, void *stream);
+/* One train-log entry: if advance_step, *step += 1 first; then row (*step % slots) of ring ((slots, 1 + n_values +
+ * n_counters) doubles) = [*step, *values[0..n_values), counters[0..n_counters)].  values: host array of device pointers to
+ * one float each (n_values <= SV_TRAIN_LOG_MAX_VALUES). */
+enum { SV_TRAIN_LOG_MAX_VALUES = 32 };
+int sv_train_log_write(int n_values, const float *const *values, const double *counters, int n_counters, long long *step,
+                       int advance_step, double *ring, int slots, void *stream);
 
 #ifdef __cplusplus
 }

@@ -20,7 +20,7 @@ AUG_ITEM_STRIDE, AUG_OBJ_STRIDE = 25, 12
 
 
 # include/svgps.h evaluation counter layouts (float64 words)
-EVAL_GROUNDING, EVAL_OBJ_CLS, EVAL_ANSWERS = 0, 1, 2
+EVAL_GROUNDING, EVAL_OBJ_CLS, EVAL_ANSWERS, EVAL_PRETRAIN = 0, 1, 2, 3
 (EVG_ITEMS, EVG_MULTIPLE, EVG_HARD, EVG_VIEW_DEP, EVG_OG_ACC, EVG_OG_ACC_HARD, EVG_OG_ACC_VIEW_DEP, EVG_IOU25, EVG_IOU50,
  EVG_IOU25_MULTIPLE, EVG_IOU50_MULTIPLE, EVG_TXT_ACC, EVG_OBJ) = range(13)
 EVG_SIZE = EVG_OBJ + 6
@@ -28,6 +28,11 @@ EVO_HIT, EVO_COUNT, EVO_SIZE = 0, 1, 2
 EVA_NTYPES = 6
 EVA_ITEMS, EVA_ANS1, EVA_ANS10, EVA_TYPE_ITEMS, EVA_TYPE_ANS1, EVA_OBJ_HIT, EVA_OBJ_COUNT = 0, 1, 2, 3, 9, 15, 16
 EVA_SNAPSHOT, EVA_Q_ANS1, EVA_Q_ANS10, EVA_Q_OBJ, EVA_Q_TYPE, EVA_Q_TYPE_COUNT, EVA_SIZE = 17, 34, 35, 36, 37, 43, 49
+EVP_OG, EVP_ITEMS, EVP_LM_HIT, EVP_LM_COUNT, EVP_OBJ, EVP_SNAPSHOT, EVP_Q, EVP_SIZE = 0, 12, 13, 14, 15, 33, 66, 76
+(EVP_Q_TARGET, EVP_Q_OG, EVP_Q_LM, EVP_Q_POST, EVP_Q_PRE, EVP_Q_RAW, EVP_Q_PRE_UNMASK, EVP_Q_PRE_MASK, EVP_Q_POST_UNMASK,
+ EVP_Q_POST_MASK) = range(10)
+EVP_HAS_OG, EVP_HAS_POST, EVP_HAS_RAW, EVP_HAS_PRE = 1, 2, 4, 8
+TRAIN_LOG_MAX_VALUES = 32
 
 
 class AugParams(ctypes.Structure):

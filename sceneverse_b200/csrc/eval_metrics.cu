@@ -1,5 +1,5 @@
-// Evaluation metrics of the fine-tuning configs reduced on the GPU (reference: evaluator/scanrefer_eval.py,
-// referit3d_eval.py, scanqa_eval.py, sqa3d_eval.py, objcls_eval.py `batch_metrics`).  Every kernel ADDS into one device
+// Evaluation metrics reduced on the GPU (reference: evaluator/scanrefer_eval.py, referit3d_eval.py, scanqa_eval.py,
+// sqa3d_eval.py, objcls_eval.py, pretrain_eval.py `batch_metrics`), and the per-step train-log write.  Every kernel ADDS into one device
 // counter vector per evaluator (float64 words, layouts in include/svgps.h), so an epoch of batches — a captured CUDA graph
 // replayed once per batch — needs no host synchronisation; `record()` reads the vector once.  Counts are integers held
 // exactly in float64 (below 2^53).  An item whose `valid` byte is 0 (padding of the last batch) counts nothing.
@@ -120,16 +120,18 @@ struct ObjClsArgs {
   long long row_stride[3], item_stride[3];
   int n, B, O, C;
   const long long *labels;
-  const unsigned char *masks, *valid;
+  const unsigned char *masks, *split, *valid;
 };
 
-// one warp per (item, object) row; hits of tensor t -> ctr[2t], masked rows -> ctr[2t + 1]
+// one warp per (item, object) row.  Without a split mask: hits of tensor t -> ctr[2t], masked rows -> ctr[2t + 1].  With
+// one: tensor t owns ctr[6t .. 6t + 5], the (hits, rows) pairs over obj_masks, obj_masks & split, obj_masks & !split.
 __global__ void __launch_bounds__(kThreads) obj_cls_kernel(ObjClsArgs a, double *__restrict__ ctr) {
   __shared__ unsigned red[kWarps];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long r = (long long)blockIdx.x * kWarps + warp;
   const int b = (int)(r / a.O), o = (int)(r % a.O);
   const bool live = r < (long long)a.B * a.O && a.masks[r] && (!a.valid || a.valid[b]);
+  const bool in_split = live && a.split && a.split[r];
 #pragma unroll
   for (int t = 0; t < 3; ++t) {
     if (t >= a.n) break;
@@ -142,10 +144,78 @@ __global__ void __launch_bounds__(kThreads) obj_cls_kernel(ObjClsArgs a, double 
     }
     const unsigned h = block_count(hit, red);
     const unsigned m = block_count(lane == 0 && live, red);
-    if (threadIdx.x == 0) {
-      if (h) atomicAdd(ctr + 2 * t, (double)h);
-      if (m) atomicAdd(ctr + 2 * t + 1, (double)m);
+    if (!a.split) {
+      if (threadIdx.x == 0) {
+        if (h) atomicAdd(ctr + 2 * t, (double)h);
+        if (m) atomicAdd(ctr + 2 * t + 1, (double)m);
+      }
+      continue;
     }
+    const unsigned hs = block_count(hit && in_split, red);
+    const unsigned ms = block_count(lane == 0 && in_split, red);
+    if (threadIdx.x == 0) {
+      double *c = ctr + 6 * t;
+      const unsigned v[6] = {h, m, hs, ms, h - hs, m - ms};
+#pragma unroll
+      for (int k = 0; k < 6; ++k)
+        if (v[k]) atomicAdd(c + k, (double)v[k]);
+    }
+  }
+}
+
+// masked-LM accuracy: one CTA per token row of (R, V) logits; rows whose label is -1 leave at once.  Labelled rows: hit when
+// the argmax over the V real columns equals the label (pad columns past V are never read).  The first row of every valid
+// item adds one item.  VEC: 16-byte loads (row pitch and base 16-byte aligned); the columns past V of the last vector are
+// skipped, so a padded row's pad columns never take part.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kThreads) lm_acc_kernel(const T *__restrict__ logits, long long rs, int V, int L,
+                                                          const long long *__restrict__ labels,
+                                                          const unsigned char *__restrict__ valid,
+                                                          double *__restrict__ ctr) {
+  __shared__ float sv[kWarps];
+  __shared__ int si[kWarps];
+  const long long r = blockIdx.x;
+  if (valid && !valid[r / L]) return;
+  if (threadIdx.x == 0 && r % L == 0) atomicAdd(ctr + SV_EVP_ITEMS, 1.0);
+  const long long label = labels[r];
+  if (label == -1) return;
+  const T *row = logits + r * rs;
+  float v = -INFINITY;
+  int i = 0x7fffffff;
+  if constexpr (VEC) {
+    constexpr int W = 16 / sizeof(T);
+    for (int j0 = threadIdx.x * W; j0 < V; j0 += kThreads * W) {
+      const uint4 q = __ldg(reinterpret_cast<const uint4 *>(row + j0));
+      float x[W];
+      if constexpr (W == 8) {
+        const __nv_bfloat162 *h = reinterpret_cast<const __nv_bfloat162 *>(&q);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 f = __bfloat1622float2(h[k]);
+          x[2 * k] = f.x, x[2 * k + 1] = f.y;
+        }
+      } else {
+        x[0] = __uint_as_float(q.x), x[1] = __uint_as_float(q.y), x[2] = __uint_as_float(q.z), x[3] = __uint_as_float(q.w);
+      }
+#pragma unroll
+      for (int k = 0; k < W; ++k)
+        if (j0 + k < V && before(x[k], j0 + k, v, i)) v = x[k], i = j0 + k;
+    }
+  } else {
+    for (int j = threadIdx.x; j < V; j += kThreads) {
+      const float x = ld(row, j);
+      if (before(x, j, v, i)) v = x, i = j;
+    }
+  }
+  warp_best(v, i);
+  const int warp = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) sv[warp] = v, si[warp] = i;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 0; w < kWarps; ++w)
+      if (before(sv[w], si[w], v, i)) v = sv[w], i = si[w];
+    if (i == label) atomicAdd(ctr + SV_EVP_LM_HIT, 1.0);
+    atomicAdd(ctr + SV_EVP_LM_COUNT, 1.0);
   }
 }
 
@@ -231,6 +301,69 @@ __global__ void sqa3d_batch_kernel(double *__restrict__ ctr) {
   for (int k = 0; k < SV_EVA_SNAPSHOT; ++k) snap[k] = ctr[k];
 }
 
+// PretrainEval.batch_metrics + update for the batch just added, in its float64 arithmetic and order: og_acc = hits / items,
+// every other accuracy hits / (count + 1e-8); target_metric = their sum in key order / their number; each sum gains
+// metric x items.  The batch is the difference of the integer counters and their snapshot.  One thread.
+__global__ void pretrain_batch_kernel(double *__restrict__ ctr, int present) {
+  double *snap = ctr + SV_EVP_SNAPSHOT, *q = ctr + SV_EVP_Q;
+  const double n = ctr[SV_EVP_ITEMS] - snap[SV_EVP_ITEMS];
+  if (n > 0.0) {
+    double sum = 0.0;
+    int keys = 0;
+    auto put = [&](int k, double v) {
+      q[k] = __dadd_rn(q[k], __dmul_rn(v, n));
+      sum = __dadd_rn(sum, v);
+      ++keys;
+    };
+    auto acc = [&](int hit) {
+      return __ddiv_rn(ctr[hit] - snap[hit], __dadd_rn(ctr[hit + 1] - snap[hit + 1], 1e-8));
+    };
+    if (present & SV_EVP_HAS_OG)
+      put(SV_EVP_Q_OG, __ddiv_rn(ctr[SV_EVP_OG + SV_EVG_OG_ACC] - snap[SV_EVP_OG + SV_EVG_OG_ACC], n));
+    put(SV_EVP_Q_LM, acc(SV_EVP_LM_HIT));
+    int t = SV_EVP_OBJ;
+    if (present & SV_EVP_HAS_POST) {
+      put(SV_EVP_Q_POST, acc(t));
+      put(SV_EVP_Q_POST_UNMASK, acc(t + 2));
+      put(SV_EVP_Q_POST_MASK, acc(t + 4));
+      t += 6;
+    }
+    if (present & SV_EVP_HAS_RAW) {
+      put(SV_EVP_Q_RAW, acc(t));
+      t += 6;
+    }
+    if (present & SV_EVP_HAS_PRE) {
+      put(SV_EVP_Q_PRE, acc(t));
+      put(SV_EVP_Q_PRE_UNMASK, acc(t + 2));
+      put(SV_EVP_Q_PRE_MASK, acc(t + 4));
+    }
+    q[SV_EVP_Q_TARGET] = __dadd_rn(q[SV_EVP_Q_TARGET], __dmul_rn(__ddiv_rn(sum, (double)keys), n));
+  }
+  for (int k = 0; k < SV_EVP_SNAPSHOT; ++k) snap[k] = ctr[k];
+}
+
+struct LogValues {
+  const float *v[SV_TRAIN_LOG_MAX_VALUES];
+};
+
+// one train-log entry: ring row (step % slots) = [step, values..., counters...]
+__global__ void train_log_kernel(LogValues vals, int nv, const double *__restrict__ ctr, int nc, long long *step, int advance,
+                                 double *__restrict__ ring, int slots) {
+  __shared__ long long s;
+  if (threadIdx.x == 0) {
+    long long k = *step;
+    if (advance) *step = ++k;
+    s = k;
+  }
+  __syncthreads();
+  double *row = ring + (s % slots) * (long long)(1 + nv + nc);
+  if (threadIdx.x == 0) row[0] = (double)s;
+#pragma unroll
+  for (int k = 0; k < SV_TRAIN_LOG_MAX_VALUES; ++k)
+    if (k < nv && threadIdx.x == k) row[1 + k] = (double)*vals.v[k];
+  for (int j = threadIdx.x; j < nc; j += blockDim.x) row[1 + nv + j] = ctr[j];
+}
+
 bool al(const void *p, uintptr_t a) { return ((uintptr_t)p % a) == 0; }
 
 }  // namespace
@@ -240,6 +373,7 @@ extern "C" int sv_eval_counters_size(int kind) {
     case SV_EVAL_GROUNDING: return SV_EVG_SIZE;
     case SV_EVAL_OBJ_CLS: return SV_EVO_SIZE;
     case SV_EVAL_ANSWERS: return SV_EVA_SIZE;
+    case SV_EVAL_PRETRAIN: return SV_EVP_SIZE;
     default: return 0;
   }
 }
@@ -271,7 +405,8 @@ extern "C" int sv_eval_grounding(const void *og3d_logits, int og_bf16, long long
 
 extern "C" int sv_eval_obj_cls(int n_logits, const void *const *logits, const int *is_bf16, const long long *row_stride,
                                const long long *item_stride, int B, int O, int C, const long long *obj_labels,
-                               const unsigned char *obj_masks, const unsigned char *valid, double *counters, void *stream) {
+                               const unsigned char *obj_masks, const unsigned char *split_mask, const unsigned char *valid,
+                               double *counters, void *stream) {
   if (n_logits < 1 || n_logits > 3 || B < 1 || O < 1 || C < 1 || !logits || !is_bf16 || !row_stride || !item_stride ||
       !obj_labels || !obj_masks || !counters || !al(obj_labels, 8) || !al(counters, 8))
     return SV_ERR_INVALID_ARG;
@@ -285,7 +420,7 @@ extern "C" int sv_eval_obj_cls(int n_logits, const void *const *logits, const in
     a.row_stride[t] = row_stride[t];
     a.item_stride[t] = item_stride[t];
   }
-  a.n = n_logits, a.B = B, a.O = O, a.C = C, a.labels = obj_labels, a.masks = obj_masks, a.valid = valid;
+  a.n = n_logits, a.B = B, a.O = O, a.C = C, a.labels = obj_labels, a.masks = obj_masks, a.split = split_mask, a.valid = valid;
   const long long rows = (long long)B * O;
   obj_cls_kernel<<<(unsigned)((rows + kWarps - 1) / kWarps), kThreads, 0, (cudaStream_t)stream>>>(a, counters);
   return sv::after_launch();
@@ -310,5 +445,46 @@ extern "C" int sv_eval_answers(const void *answer_scores, int is_bf16, long long
 extern "C" int sv_eval_sqa3d_batch(double *counters, void *stream) {
   if (!counters || !al(counters, 8)) return SV_ERR_INVALID_ARG;
   sqa3d_batch_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(counters);
+  return sv::after_launch();
+}
+
+extern "C" int sv_eval_lm_acc(const void *logits, int is_bf16, long long row_stride, long long R, int V, int L,
+                              const long long *masked_lm_labels, const unsigned char *valid, double *counters, void *stream) {
+  if (R < 1 || V < 1 || L < 1 || R % L || row_stride < V || !logits || !masked_lm_labels || !counters) return SV_ERR_INVALID_ARG;
+  if (R > 0x7fffffffLL || !al(logits, is_bf16 ? 2 : 4) || !al(masked_lm_labels, 8) || !al(counters, 8)) return SV_ERR_INVALID_ARG;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int es = is_bf16 ? 2 : 4;
+  const bool vec = al(logits, 16) && (row_stride * es) % 16 == 0;
+  const unsigned grid = (unsigned)R;
+  if (is_bf16) {
+    const __nv_bfloat16 *p = (const __nv_bfloat16 *)logits;
+    if (vec) lm_acc_kernel<__nv_bfloat16, true><<<grid, kThreads, 0, st>>>(p, row_stride, V, L, masked_lm_labels, valid, counters);
+    else lm_acc_kernel<__nv_bfloat16, false><<<grid, kThreads, 0, st>>>(p, row_stride, V, L, masked_lm_labels, valid, counters);
+  } else {
+    const float *p = (const float *)logits;
+    if (vec) lm_acc_kernel<float, true><<<grid, kThreads, 0, st>>>(p, row_stride, V, L, masked_lm_labels, valid, counters);
+    else lm_acc_kernel<float, false><<<grid, kThreads, 0, st>>>(p, row_stride, V, L, masked_lm_labels, valid, counters);
+  }
+  return sv::after_launch();
+}
+
+extern "C" int sv_eval_pretrain_batch(double *counters, int present, void *stream) {
+  if (!counters || !al(counters, 8) || (present & ~(SV_EVP_HAS_OG | SV_EVP_HAS_POST | SV_EVP_HAS_RAW | SV_EVP_HAS_PRE)))
+    return SV_ERR_INVALID_ARG;
+  pretrain_batch_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(counters, present);
+  return sv::after_launch();
+}
+
+extern "C" int sv_train_log_write(int n_values, const float *const *values, const double *counters, int n_counters,
+                                  long long *step, int advance_step, double *ring, int slots, void *stream) {
+  if (n_values < 0 || n_values > SV_TRAIN_LOG_MAX_VALUES || n_counters < 0 || slots < 1 || !step || !ring ||
+      (n_values && !values) || (n_counters && !counters) || !al(step, 8) || !al(ring, 8) || !al(counters, 8))
+    return SV_ERR_INVALID_ARG;
+  LogValues v{};
+  for (int k = 0; k < n_values; ++k) {
+    if (!values[k] || !al(values[k], 4)) return SV_ERR_INVALID_ARG;
+    v.v[k] = values[k];
+  }
+  train_log_kernel<<<1, 128, 0, (cudaStream_t)stream>>>(v, n_values, counters, n_counters, step, advance_step, ring, slots);
   return sv::after_launch();
 }

@@ -1,11 +1,12 @@
-"""Evaluation of the fine-tuning configs (reference: evaluator/build.py:10-53 `BaseEvaluator`, scanrefer_eval.py,
-referit3d_eval.py, scanqa_eval.py, sqa3d_eval.py, objcls_eval.py; trainer/openvocab_trainer.py:48-62 `eval_step`).
+"""Evaluation (reference: evaluator/build.py:10-53 `BaseEvaluator`, scanrefer_eval.py, referit3d_eval.py, scanqa_eval.py,
+sqa3d_eval.py, objcls_eval.py, pretrain_eval.py; trainer/openvocab_trainer.py:48-62 `eval_step`).
 
 Each evaluator keeps its metrics as one float64 counter vector on the device (layouts: include/svgps.h SV_EV*).  `update`
 launches the metric kernels of csrc/eval_metrics.cu, which add one batch into it: no host synchronisation, so the updates of
 an epoch can be replayed from a CUDA graph (`EvalRunner`).  `record` reads the vector once (after one all_reduce(SUM) when
 several ranks evaluate) and builds the reference's dictionary: integer totals divided by counts, or, for SQA3DEval, its
 batch-size-weighted average of per-batch ratios, accumulated on the device in the reference's float64 order.
+`counts_to_metrics` turns one batch's counter values into `batch_metrics`; train.PretrainStep's per-step logs use it too.
 
 Not supported (NotImplementedError): `cfg.eval.save` (results.json) and per-scene (3-D) grounding logits.
 An item whose `valid` entry is False (the padding of a last partial batch) counts nothing."""
@@ -16,7 +17,7 @@ import torch.distributed as dist
 
 from . import _lib
 
-__all__ = ["ScanReferEval", "ReferIt3DEval", "ScanQAEval", "SQA3DEval", "PretrainObjEval", "EvalRunner"]
+__all__ = ["ScanReferEval", "ReferIt3DEval", "ScanQAEval", "SQA3DEval", "PretrainObjEval", "PretrainEval", "EvalRunner"]
 
 
 def _is_bf16(t):
@@ -58,8 +59,9 @@ def _obj_logit_keys(data_dict):
             and v.shape[:2] == shape]
 
 
-def _launch_obj_cls(tensors, data_dict, valid, counters):
-    """Masked-argmax hits of up to three (B, O, C) logits tensors; pairs (hits, count) from counters[0]."""
+def _launch_obj_cls(tensors, data_dict, valid, counters, split=None):
+    """Masked-argmax hits of up to three (B, O, C) logits tensors; pairs (hits, count) from counters[0], or with a (B, O)
+    split mask three pairs per tensor (all masked objects, those in the split, those outside it)."""
     labels = _i64(data_dict["obj_labels"], "obj_labels")
     masks = _bytes(data_dict["obj_masks"])
     B, O, C = tensors[0].shape
@@ -73,8 +75,10 @@ def _launch_obj_cls(tensors, data_dict, valid, counters):
     bf = arr(ctypes.c_int, [_is_bf16(t) for t in tensors])
     rs = arr(ctypes.c_longlong, [t.stride(1) for t in tensors])
     its = arr(ctypes.c_longlong, [t.stride(0) for t in tensors])
+    if split is not None and tuple(split.shape) != (B, O):
+        raise ValueError(f"the split mask must be {(B, O)}, got {tuple(split.shape)}")
     _lib.call(_lib.gps(), "sv_eval_obj_cls", labels.device, n, ptrs, bf, rs, its, B, O, C, labels.data_ptr(), masks.data_ptr(),
-              _lib.ptr(valid), counters.data_ptr())
+              _lib.ptr(split), _lib.ptr(valid), counters.data_ptr())
 
 
 class _CounterEvaluator:
@@ -112,7 +116,12 @@ class _CounterEvaluator:
         return c.tolist()
 
     def batch_metrics(self, data_dict, include_count=False):
-        metrics = self._metrics(self._batch_counts(data_dict))
+        return self.counts_to_metrics(self._batch_counts(data_dict), include_count)
+
+    def counts_to_metrics(self, c, include_count=False):
+        """`batch_metrics` of one batch from its counter values `c` (a list of floats): the one host arithmetic shared by the
+        eager `batch_metrics` and the per-step train logs (train.PretrainStep.logs)."""
+        metrics = self._metrics(c)
         if not include_count:
             return {k: v[0] / max(v[1], 1) for k, v in metrics.items()}
         return metrics
@@ -303,7 +312,9 @@ class SQA3DEval(_CounterEvaluator):
         _lib.call(_lib.gps(), "sv_eval_sqa3d_batch", counters.device, counters.data_ptr())
 
     def batch_metrics(self, data_dict):
-        c = self._batch_counts(data_dict)
+        return self.counts_to_metrics(self._batch_counts(data_dict))
+
+    def counts_to_metrics(self, c, include_count=False):
         n = int(c[_lib.EVA_ITEMS])
         m = {"ans1_acc": c[_lib.EVA_ANS1] / float(n), "ans10_acc": c[_lib.EVA_ANS10] / float(n),
              "obj_cls_raw_acc": c[_lib.EVA_OBJ_HIT] / float(c[_lib.EVA_OBJ_COUNT])}
@@ -326,6 +337,96 @@ class SQA3DEval(_CounterEvaluator):
                 self.eval_dict[k] = c[_lib.EVA_Q_TYPE + int(k[4])] / c[_lib.EVA_Q_TYPE_COUNT + int(k[4])]
             else:
                 self.eval_dict[k] = sums[k] / total
+        is_best = self.eval_dict["target_metric"] > self.best_result
+        if is_best:
+            self.best_result = self.eval_dict["target_metric"]
+        return is_best, self.eval_dict
+
+
+def _sum_left_to_right(xs):
+    """The builtin sum of the reference's Python 3.9: one rounded addition per item, in order (from Python 3.12 on, sum()
+    compensates the rounding)."""
+    total = 0
+    for x in xs:
+        total = total + x
+    return total
+
+
+class PretrainEval(_CounterEvaluator):
+    """evaluator/pretrain_eval.py: og_acc, lang_cls_acc_mask (masked-LM accuracy over the tokens whose masked_lm_labels is not
+    -1) and obj_cls_{post,raw,pre}_acc, the post / pre ones also over obj_masks & obj_sem_masks (`_unmask`) and
+    obj_masks & ~obj_sem_masks (`_mask`); each key only if its input is in the batch.  Its arithmetic is kept as it is:
+    og_acc = hits / B with no mask (the plain einsum's padded slots can win), every other accuracy hits / (count + 1e-8)
+    (0.0 for a batch with no labelled token), target_metric = the mean of the batch's accuracies.  `update` stores metric x
+    total_count per batch and `record` divides the sums by the total count (a key never seen records 0.0); the device keeps
+    exactly those float64 sums (sv_eval_pretrain_batch after every batch), so `record` returns the reference's values.  Sums
+    are left to right, as the builtin sum of the reference's pinned Python 3.9 adds them."""
+    kind = _lib.EVAL_PRETRAIN
+    target_metric = "target_metric"
+    KEYS = ["target_metric", "og_acc", "lang_cls_acc_mask", "obj_cls_post_acc", "obj_cls_pre_acc", "obj_cls_raw_acc",
+            "obj_cls_pre_acc_unmask", "obj_cls_pre_acc_mask", "obj_cls_post_acc_unmask", "obj_cls_post_acc_mask"]
+    OBJ = (("obj_cls_post_logits", _lib.EVP_HAS_POST), ("obj_cls_raw_logits", _lib.EVP_HAS_RAW),
+           ("obj_cls_pre_logits", _lib.EVP_HAS_PRE))
+
+    def __init__(self, *a, **k):
+        self.present = 0           # SV_EVP_HAS_* bits of the last batch: which keys batch_metrics reports
+        super().__init__(*a, **k)
+
+    def _launch(self, data_dict, valid, counters):
+        lm = data_dict["txt_lm_cls_logits"]
+        labels = _i64(data_dict["masked_lm_labels"], "masked_lm_labels")
+        if lm.dim() != 3 or lm.stride(2) != 1 or lm.stride(0) != lm.shape[1] * lm.stride(1):
+            raise ValueError("txt_lm_cls_logits must be (B, L, V) with unit stride along V and rows of one pitch, got shape "
+                             f"{tuple(lm.shape)} strides {lm.stride()}")
+        B, L, V = lm.shape
+        if tuple(labels.shape) != (B, L):
+            raise ValueError(f"masked_lm_labels must be {(B, L)}, got {tuple(labels.shape)}")
+        present = 0
+        if "tgt_object_id" in data_dict:
+            og = data_dict["og3d_logits"]
+            if og.dim() != 2 or og.shape[0] != B:
+                raise ValueError(f"og3d_logits must be ({B}, O), got {tuple(og.shape)}")
+            tgt = _i64(data_dict["tgt_object_id"], "tgt_object_id").reshape(-1)
+            _lib.call(_lib.gps(), "sv_eval_grounding", og.device, og.data_ptr(), _is_bf16(og), og.stride(0), og.stride(1), B,
+                      og.shape[1], tgt.data_ptr(), None, None, 0, None, 0, 0, 0, None, None, None, None, _lib.ptr(valid),
+                      counters[_lib.EVP_OG:].data_ptr())
+            present |= _lib.EVP_HAS_OG
+        obj = [(k, bit) for k, bit in self.OBJ if k in data_dict]
+        if obj:
+            present |= sum(bit for _, bit in obj)
+            # the split is only reported for post / pre; raw alone needs no obj_sem_masks
+            sem = data_dict["obj_sem_masks"] if present & (_lib.EVP_HAS_POST | _lib.EVP_HAS_PRE) else \
+                data_dict.get("obj_sem_masks", data_dict["obj_masks"])
+            _launch_obj_cls([data_dict[k] for k, _ in obj], data_dict, valid, counters[_lib.EVP_OBJ:], split=_bytes(sem))
+        _lib.call(_lib.gps(), "sv_eval_lm_acc", lm.device, lm.data_ptr(), _is_bf16(lm), lm.stride(1), B * L, V, L,
+                  labels.data_ptr(), _lib.ptr(valid), counters.data_ptr())
+        _lib.call(_lib.gps(), "sv_eval_pretrain_batch", counters.device, counters.data_ptr(), present)
+        self.present = present
+
+    def counts_to_metrics(self, c, include_count=False):
+        n = int(c[_lib.EVP_ITEMS])
+        acc = lambda k: int(c[k]) / float(int(c[k + 1]) + 1e-8)  # noqa: E731
+        m = {}
+        if self.present & _lib.EVP_HAS_OG:
+            m["og_acc"] = int(c[_lib.EVP_OG + _lib.EVG_OG_ACC]) / float(n)
+        m["lang_cls_acc_mask"] = acc(_lib.EVP_LM_HIT)
+        t = _lib.EVP_OBJ
+        for name, bit in ((k[:-len("logits")], b) for k, b in self.OBJ):
+            if self.present & bit:
+                m[name + "acc"] = acc(t)
+                if bit != _lib.EVP_HAS_RAW:
+                    m[name + "acc_unmask"] = acc(t + 2)
+                    m[name + "acc_mask"] = acc(t + 4)
+                t += 6
+        all_acc = list(m.values())
+        m["target_metric"] = float(_sum_left_to_right(all_acc)) / len(all_acc)
+        m["total_count"] = n
+        return m
+
+    def record(self):
+        c = self._reduced()
+        total = int(c[_lib.EVP_ITEMS])
+        self.eval_dict = {k: c[_lib.EVP_Q + i] / total for i, k in enumerate(self.KEYS)}
         is_best = self.eval_dict["target_metric"] > self.best_result
         if is_best:
             self.best_result = self.eval_dict["target_metric"]

@@ -30,21 +30,97 @@ class StepModule(nn.Module):
         for n, p in self.model.named_parameters():
             if n.startswith(STATIC_UNUSED):
                 p.requires_grad = False
+        self.train_log = None      # TrainLog of PretrainStep(train_eval=...): written after the losses, before backward
 
     def forward(self, data_dict):
         data_dict = self.model(data_dict)
         total, all_losses = self.loss(data_dict)
+        if self.train_log is not None:
+            self.train_log.write(data_dict, all_losses)
         return total, all_losses
+
+
+class TrainLog:
+    """The per-step train log of trainer/openvocab_trainer.py:26-46 without a host synchronisation per step.  Inside the step
+    (captured in the CUDA graph), right after the losses, the evaluator's metric kernels add the batch into a per-step counter
+    vector zeroed first, and one native write (sv_train_log_write) copies the device step, every loss-dict value and those
+    counters into row (step % slots) of a device ring.  `read` copies the ring to the host once and builds one dictionary per
+    step since the previous read with the evaluator's own count -> metric arithmetic (`counts_to_metrics`)."""
+
+    def __init__(self, evaluator, loss_keys, slots, device):
+        from . import _lib
+        if slots < 1:
+            raise ValueError(f"log_every must be at least 1, got {slots}")
+        if len(loss_keys) > _lib.TRAIN_LOG_MAX_VALUES:
+            raise ValueError(f"at most {_lib.TRAIN_LOG_MAX_VALUES} loss-dict entries can be logged, got {len(loss_keys)}")
+        self.evaluator = evaluator
+        self.loss_keys = list(loss_keys)
+        self.slots = int(slots)
+        self.counters = torch.zeros(evaluator.size, dtype=torch.float64, device=device)
+        self.ring = torch.zeros((self.slots, 1 + len(self.loss_keys) + evaluator.size), dtype=torch.float64, device=device)
+        self.own_step = torch.zeros(1, dtype=torch.int64, device=device)
+        self.step_counter, self.advance = self.own_step, True    # eager: the write advances its own counter
+        self.seen = 0          # device step of the newest entry already read (or discarded)
+        self.pending = []      # (train/step, [lr of each group]) of the steps not read yet, in order
+
+    def write(self, data_dict, all_losses):
+        from . import _lib
+        import ctypes
+        if list(all_losses) != self.loss_keys:
+            raise ValueError(f"loss-dict keys {list(all_losses)} differ from the logged {self.loss_keys}")
+        with torch.no_grad():
+            self.counters.zero_()
+            try:
+                self.evaluator._launch(data_dict, None, self.counters)
+            except KeyError as e:
+                raise KeyError(f"{type(self.evaluator).__name__} needs {e.args[0]!r}, which the step's data dict lacks") from None
+            vals = [v.detach().reshape(()) if v.dtype == torch.float32 else v.detach().float().reshape(())
+                    for v in all_losses.values()]
+            ptrs = (ctypes.c_void_p * len(vals))(*[v.data_ptr() for v in vals])
+            _lib.call(_lib.gps(), "sv_train_log_write", self.ring.device, len(vals), ptrs, self.counters.data_ptr(),
+                      self.counters.numel(), self.step_counter.data_ptr(), int(self.advance), self.ring.data_ptr(), self.slots)
+
+    def begin_step(self):
+        if len(self.pending) >= self.slots:
+            raise RuntimeError(f"{len(self.pending)} steps since the last logs() call fill the log ring (log_every = "
+                               f"{self.slots}): call logs() at least every log_every steps")
+
+    def end_step(self, step, lrs):
+        self.pending.append((step, list(lrs)))
+
+    def read(self):
+        if not self.pending:
+            return []
+        ring = self.ring.cpu().tolist()                        # the one device-to-host copy
+        rows = sorted((r for r in ring if r[0] > self.seen), key=lambda r: r[0])
+        if len(rows) != len(self.pending):
+            raise RuntimeError(f"the log ring holds {len(rows)} new entries for {len(self.pending)} steps")
+        nl = len(self.loss_keys)
+        out = []
+        for row, (step, lrs) in zip(rows, self.pending):
+            d = {"train/step": step}
+            d.update((f"train/{k}", v) for k, v in zip(self.loss_keys, row[1:1 + nl]))
+            d.update((f"train/{k}", v) for k, v in self.evaluator.counts_to_metrics(row[1 + nl:]).items())
+            d.update((f"train/lr/group_{i}", lr) for i, lr in enumerate(lrs))
+            out.append(d)
+        self.seen = rows[-1][0]
+        self.pending = []
+        return out
 
 
 class PretrainStep:
     def __init__(self, cfg, device, total_steps=100000, dtype=torch.bfloat16, ddp=None, seed=0, cuda_graph=False,
-                 overlap_allreduce=False):
+                 overlap_allreduce=False, train_eval=None, log_every=100):
         """cuda_graph=True (single process, CUDA): after a few eager steps the whole step — forward, losses, backward,
         gradient clipping and AdamW — is captured once into a CUDA graph and replayed from static input buffers; the host
         then issues one graph launch per step instead of ~2000 kernel launches.  Dropout stays random: torch's own dropout
         through the graph-registered generator, the in-kernel masks through the device step counter registered with
-        sv_dropout_seed_offset."""
+        sv_dropout_seed_offset.
+
+        train_eval (an evaluator of sceneverse_b200.evaluate: PretrainEval, ScanReferEval, ReferIt3DEval, ScanQAEval or
+        SQA3DEval): every step also records its loss dict and the evaluator's counts on the device, inside the graph, and
+        `logs()` returns them as the reference trainer's per-step log dictionaries.  log_every: the ring's size; more steps
+        than that between two `logs()` calls raise.  None (the default) leaves the step as it is without logs."""
         torch.manual_seed(seed)
         self.cfg = M.to_cfg(cfg)
         self.device = torch.device(device)
@@ -93,14 +169,39 @@ class PretrainStep:
         self.ddp = None
         self.probed = False
         self.module.train()
+        self.global_step = 0
+        self.train_log = None
+        if train_eval is not None:
+            self.train_log = TrainLog(train_eval, list(self.module.loss.loss_fn) + ["total_loss"], log_every, self.device)
+            if self.graph_mode:    # the graph's own step counter indexes the ring
+                self.train_log.step_counter, self.train_log.advance = self._step_counter, False
+            self.module.train_log = self.train_log
+
+    def logs(self):
+        """One dictionary per step since the previous call, in order, with the reference trainer's keys (`train/step`,
+        `train/<loss>` for every loss-dict entry and `train/total_loss`, `train/<metric>` of the evaluator's batch_metrics,
+        `train/lr/group_i`), ready for accelerator.log; one device-to-host copy.  Needs train_eval."""
+        if self.train_log is None:
+            raise RuntimeError("PretrainStep was built without train_eval: there are no logs")
+        return self.train_log.read()
+
+    def _lrs(self):
+        if self.scheduler is not None:
+            return self.scheduler.get_last_lr()
+        f = self._lr_lambda(self._sched_step)
+        return [base * f for base in self._base_lrs]
 
     def _probe_unused(self, data_dict):
         """One local forward/backward to find the parameters this configuration never touches (e.g. the object LM head
         when `obj_cls_post_logits` is in no loss, all_pretrain.yaml:246-258).  They are frozen once, so DDP can run with
         find_unused_parameters=False instead of the reference's per-step graph search (trainer/build.py:66)."""
         self.optimizer.zero_grad(set_to_none=True)
-        with torch.autocast(self.device.type, dtype=self.dtype, enabled=self.dtype != torch.float32):
-            total, _ = self.module(dict(data_dict))
+        log, self.module.train_log = self.module.train_log, None      # not a training step: nothing to log
+        try:
+            with torch.autocast(self.device.type, dtype=self.dtype, enabled=self.dtype != torch.float32):
+                total, _ = self.module(dict(data_dict))
+        finally:
+            self.module.train_log = log
         total.backward()
         unused = [n for n, p in self.module.named_parameters() if p.requires_grad and p.grad is None]
         for n, p in self.module.named_parameters():
@@ -278,6 +379,8 @@ class PretrainStep:
                               "using graph | all-reduce | graph")
                 finally:
                     self._overlap_now = False
+        if self.train_log is not None:          # the eager set-up steps' entries are not steps of the run
+            self.train_log.seen = int(self._step_counter.item())
 
     def _dp_graph_possible(self):
         """Graph A must not contain an NCCL collective: with several ranks the contrastive exchange has to be the native
@@ -294,7 +397,9 @@ class PretrainStep:
                 self.ddp = nn.parallel.DistributedDataParallel(
                     self.module, device_ids=[self.device.index], find_unused_parameters=False,
                     gradient_as_bucket_view=True, bucket_cap_mb=64)
-                return self.step(data_dict)
+                if self.train_log is not None:
+                    self.train_log.step_counter, self.train_log.advance = self.train_log.own_step, True
+                return self._step(data_dict)
         if self.graph is None:
             self._capture(data_dict)
         for k, dst in self.static_batch.items():
@@ -342,6 +447,15 @@ class PretrainStep:
         i.e. four parameter updates on that batch, unlike the reference's one step per batch; feed a throw-away batch first if
         that matters.  (2) the returned tensor is the graph's STATIC loss buffer, overwritten by the next replay: read it
         (`.item()` / `.clone()`) before calling step() again if the value has to be kept."""
+        if self.train_log is not None:
+            self.train_log.begin_step()
+        loss = self._step(data_dict)
+        self.global_step += 1
+        if self.train_log is not None:
+            self.train_log.end_step(self.global_step, self._lrs())
+        return loss
+
+    def _step(self, data_dict):
         if self.graph_mode:
             return self._graph_step(data_dict)
         if not self.probed:
