@@ -7,12 +7,13 @@
 //     reference are never materialised;
 //   * nn.MultiheadAttention's scaled-dot-product core incl. its attention-weight dropout (joint self-attention of
 //     UnifiedSpatialCrossEncoderV2, self/cross attention of the V1 / Entity decoders; transformers.py:22-24,69-74,118-120).
-// One CTA = one (scene, head), two warpgroups; each owns 64 of the 128 query rows of a tile.  Q / K / V head slices arrive
-// by TMA (128-byte swizzle, zero-filled past the sequence end).  The softmax takes two passes over 64-key blocks of
-// S = Q K^T, each block one wgmma chain into 32 registers per thread: pass 1 finds the row maximum, pass 2 recomputes the
-// block, exponentiates, sums and writes the unnormalised bf16 probabilities P to shared memory as the K-major A operand
-// of O = P V, whose B operand is the SAME staged V tile read MN-major (no transposed copy).  1 / sum is applied to the
-// fp32 output row.  Exactly the two-pass arithmetic of a full-row softmax: no online rescaling.
+// One CTA = one warpgroup = one unit (scene, head, 64 query rows); Q / K / V head slices arrive by TMA (128-byte swizzle,
+// zero-filled past the sequence end).  The softmax takes two passes over 64-key blocks of S = Q K^T, each block one wgmma
+// chain into 32 registers per thread: pass 1 finds the row maximum, pass 2 recomputes the block, exponentiates, sums and
+// writes the block's unnormalised bf16 probabilities P to shared memory (two buffers, even / odd blocks) as the K-major A
+// operand of O += P V, whose B operand is the SAME staged V tile read MN-major (no transposed copy); that chain is left in
+// flight behind the next block's S chain.  1 / sum is applied to the fp32 output row.  Exactly the two-pass arithmetic of a
+// full-row softmax: no online rescaling.
 #include "attn_common.cuh"
 #include "svgps.h"
 
@@ -36,176 +37,176 @@ struct FwdArgs {
   const unsigned long long *seed_offset;  // device counter added to the seed at run time (or null)
 };
 
-// S block = Q rows [64 wg, 64 wg + 64) x keys [k0, k0 + 64): 4 K = 16 steps over the head dims
-__device__ __forceinline__ void s_block(float (&s)[32], uint32_t aQ, uint32_t aK) {
-  wgmma_fence();
-#pragma unroll
-  for (int ks = 0; ks < DH / 16; ++ks) wgmma_n64<0, 0>(s, desc_sw128(aQ + ks * 32, 16), desc_sw128(aK + ks * 32, 16), ks > 0);
-  wgmma_commit();
-  wgmma_wait<0>();
-  fence_regs(s);
-}
-
 template <bool GATED, bool DROP>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(128, 3)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ CUtensorMap mk,
                 const __grid_constant__ CUtensorMap mv, const FwdArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int NK = (a.Lk + 15) & ~15;          // keys rounded to the TMA box
-  const int NK64 = (a.Lk + 63) & ~63;        // keys rounded to the 64-key blocks of S
+  const int NK64 = (a.Lk + 63) & ~63;        // keys rounded to the 64-key blocks
   const int nkbox = NK >> 4;                 // 16-row TMA boxes of K / V
-  uint8_t *sQ = smem;                        // [128][64] sw128
-  uint8_t *sK = sQ + 16384;                  // [NK64][64] sw128
-  uint8_t *sV = sK + NK64 * 128;             // [NK64][64] sw128 (read MN-major)
-  uint8_t *sP = sV + NK64 * 128;             // [NK64/8][128][8] K-major, no swizzle
-  float *kb = reinterpret_cast<float *>(sP + NK64 * 256);  // [NK64] additive key bias: 0 or -inf
-  uint64_t *bars = reinterpret_cast<uint64_t *>(kb + 384);  // 0: K/V landed, 1: Q tile landed
+  const int nblk = NK64 >> 6;                // 64-key blocks, the element-wise work of the last one NK - 64 (nblk - 1) wide
+  uint8_t *sQ = smem;                        // [64][64] sw128
+  uint8_t *sK = sQ + 8192;                   // [NK][64] sw128 (the S columns of keys past NK are never read)
+  uint8_t *sV = sK + NK * 128;               // [NK64][64] sw128 (read MN-major)
+  uint8_t *sP = sV + NK64 * 128;             // 2 x [8][64][8] K-major, no swizzle: P of the even / odd key blocks
+  float *kb = reinterpret_cast<float *>(sP + 16384);        // [nblk * 64] additive key bias: 0 or -inf
+  uint64_t *bar = reinterpret_cast<uint64_t *>(kb + 384);  // Q, K and V landed
 
-  const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127, w = t >> 5, lane = tid & 31;
-  const int rl = wg * 64 + w * 16 + (lane >> 2);   // this thread's first row in the tile (second: rl + 8)
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+  const int rl = w * 16 + (lane >> 2);             // this thread's first row in the tile (second: rl + 8)
   const int cq = 2 * (lane & 3);                   // its first column in every 8-column group
-  const int b = blockIdx.x / a.H, h = blockIdx.x % a.H;
+  const int nqt = (a.Lq + 63) >> 6;
+  const int bh = blockIdx.x / nqt, q0 = (blockIdx.x % nqt) * 64;
+  const int b = bh / a.H, h = bh % a.H;
 
   if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
+    mbar_init(bar, 1);
     mbar_fence_init();
   }
-  // key rows [NK, NK64) of K and V are never written by TMA: zero them so padded S columns / P.V terms are exact zeros
-  for (int i = tid; i < (NK64 - NK) * 8; i += 256) {
-    reinterpret_cast<uint4 *>(sK + NK * 128)[i] = make_uint4(0, 0, 0, 0);
-    reinterpret_cast<uint4 *>(sV + NK * 128)[i] = make_uint4(0, 0, 0, 0);
-  }
-  for (int j = tid; j < NK64; j += 256)
+  // V rows [NK, NK64) are never written by TMA: zero them so that the P V terms of the padded keys are exact zeros
+  for (int i = tid; i < (NK64 - NK) * 8; i += 128) reinterpret_cast<uint4 *>(sV + NK * 128)[i] = make_uint4(0, 0, 0, 0);
+  for (int j = tid; j < NK64; j += 128)
     kb[j] = (j < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + j])) ? 0.f : -INFINITY;
   fence_proxy_async_smem();
   __syncthreads();
   if (tid == 0) {
-    mbar_expect_tx(&bars[0], 2 * rows_bytes(0, nkbox, a.Lk));
-    tma_rows(sK, &mk, h, 0, nkbox, a.Lk, b, &bars[0]);
-    tma_rows(sV, &mv, h, 0, nkbox, a.Lk, b, &bars[0]);
+    mbar_expect_tx(bar, rows_bytes(q0, 4, a.Lq) + 2 * rows_bytes(0, nkbox, a.Lk));
+    tma_rows(sQ, &mq, h, q0, 4, a.Lq, b, bar);
+    tma_rows(sK, &mk, h, 0, nkbox, a.Lk, b, bar);
+    tma_rows(sV, &mv, h, 0, nkbox, a.Lk, b, bar);
   }
-  mbar_wait(&bars[0], 0);
   const float c2 = a.scale * LOG2E;
-  const uint32_t aQ = smem_u32(sQ) + wg * 8192, aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(sP) + wg * 1024;
+  const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(sP);
   const unsigned long long seed = DROP ? attn::effective_seed(a.seed, a.seed_offset) : 0ull;
-  uint32_t ph_q = 0;
+  int qi[2];
+  bool qlive[2];
+  GateW gw[2];
+  const float *loc[2] = {nullptr, nullptr};
+  uint32_t rk[2] = {0u, 0u};
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    qi[r] = q0 + rl + 8 * r;
+    qlive[r] = qi[r] < a.Lq;
+    if (GATED && qlive[r]) {
+      gw[r].load(a.sw + ((size_t)b * a.Lq + qi[r]) * (a.SH * 6) + (a.SH == 1 ? 0 : h) * 6);
+      loc[r] = a.locs + ((size_t)b * a.Lq + qi[r]) * (size_t)a.Lk * 5;
+    }
+    if (DROP) rk[r] = drop_row_key(seed, ((unsigned long long)b * a.H + h) * a.Lq + qi[r]);
+  }
+  mbar_wait(bar, 0);
 
-  for (int q0 = 0; q0 < a.Lq; q0 += 128) {
-    if (tid == 0) {
-      mbar_expect_tx(&bars[1], rows_bytes(q0, 8, a.Lq));
-      tma_rows(sQ, &mq, h, q0, 8, a.Lq, b, &bars[1]);
-    }
-    mbar_wait(&bars[1], ph_q);
-    ph_q ^= 1u;
-    int qi[2];
-    bool qlive[2];
-    GateW gw[2];
-    const float *loc[2] = {nullptr, nullptr};
-    uint32_t rk[2] = {0u, 0u};
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      qi[r] = q0 + rl + 8 * r;
-      qlive[r] = qi[r] < a.Lq;
-      if (GATED && qlive[r]) {
-        gw[r].load(a.sw + ((size_t)b * a.Lq + qi[r]) * (a.SH * 6) + (a.SH == 1 ? 0 : h) * 6);
-        loc[r] = a.locs + ((size_t)b * a.Lq + qi[r]) * (size_t)a.Lk * 5;
-      }
-      if (DROP) rk[r] = drop_row_key(seed, ((unsigned long long)b * a.H + h) * a.Lq + qi[r]);
-    }
-
-    // ---- pass 1: row maximum of the scaled, masked logits (the gate is <= 0, so this bounds the gated logits too) ----
-    float m2[2] = {-INFINITY, -INFINITY};
-    for (int k0 = 0; k0 < NK64; k0 += 64) {
-      float s[32];
-      s_block(s, aQ, aK + k0 * 128);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float2 k2 = *reinterpret_cast<const float2 *>(kb + k0 + 8 * j + cq);
-#pragma unroll
-        for (int r = 0; r < 2; ++r)
-          m2[r] = fmaxf(m2[r], fmaxf(fmaf(s[4 * j + 2 * r], c2, k2.x), fmaf(s[4 * j + 2 * r + 1], c2, k2.y)));
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      m2[r] = fmaxf(m2[r], __shfl_xor_sync(0xffffffffu, m2[r], 1));
-      m2[r] = fmaxf(m2[r], __shfl_xor_sync(0xffffffffu, m2[r], 2));
-      if (m2[r] == -INFINITY) m2[r] = 0.f;  // every key masked: all weights 0, output row 0
-    }
-
-    // ---- pass 2: p = 2^(x - max), row sum, dropout, bf16 P tile -------------------------------------------------------
-    float sum[2] = {0.f, 0.f};
-    for (int k0 = 0; k0 < NK64; k0 += 64) {
-      float s[32];
-      s_block(s, aQ, aK + k0 * 128);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int col = k0 + 8 * j + cq;
-        const float2 k2 = *reinterpret_cast<const float2 *>(kb + col);
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          float x0 = fmaf(s[4 * j + 2 * r], c2, k2.x) - m2[r], x1 = fmaf(s[4 * j + 2 * r + 1], c2, k2.y) - m2[r];
-          if (GATED && loc[r] != nullptr) {
-            if (col < a.Lk) {
-              const float *l = loc[r] + (size_t)col * 5;
-              x0 += gw[r].log2gate(__ldg(l), __ldg(l + 1), __ldg(l + 2), __ldg(l + 3), __ldg(l + 4));
-            }
-            if (col + 1 < a.Lk) {
-              const float *l = loc[r] + (size_t)(col + 1) * 5;
-              x1 += gw[r].log2gate(__ldg(l), __ldg(l + 1), __ldg(l + 2), __ldg(l + 3), __ldg(l + 4));
-            }
-          }
-          float p0 = ex2f(x0), p1 = ex2f(x1);
-          sum[r] += p0 + p1;
-          if (DROP) {
-            const uint32_t hh = drop_pair_hash(rk[r], (uint32_t)col >> 1);
-            p0 = (hh & 0xFFFFu) >= a.t16 ? p0 * a.inv_keep : 0.f;
-            p1 = (hh >> 16) >= a.t16 ? p1 * a.inv_keep : 0.f;
-          }
-          // unnormalised probabilities -> bf16 A operand; 1 / sum is applied to the fp32 output row
-          *reinterpret_cast<uint32_t *>(sP + tile_off(128, rl + 8 * r, col)) = pack_bf16(p0, p1);
-        }
-      }
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 1);
-      sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 2);
-    }
-    fence_proxy_async_smem();
-    wg_sync(1 + wg);   // this warpgroup's 64 rows of P are complete
-
-    // ---- O = P V (V staged once, read MN-major) ------------------------------------------------------------------------
-    float o[32];
+  // S block blk = Q . K[64 blk, 64 blk + 64)^T, issued behind whatever chain is still in flight and waited on
+  auto s_block = [&](float (&s)[32], int blk) {
     wgmma_fence();
-    for (int ks = 0; ks < NK64 / 16; ++ks)
-      wgmma_n64<0, 1>(o, desc_noswz(aP + ks * 4096, 2048, 128), desc_sw128(aV + ks * 2048, 8192), ks > 0);
+    mma_kk(s, aQ, aK + blk * 8192);
     wgmma_commit();
     wgmma_wait<0>();
-    fence_regs(o);
+    fence_regs(s);
+  };
+  float s[32];
+
+  // ---- pass 1: row maximum of the scaled, masked logits (the gate is <= 0, so this bounds the gated logits too) ------
+  float m2[2] = {-INFINITY, -INFINITY};
+  auto row_max = [&](int blk) {
+    const int n = block_cols(blk, NK);
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      if (!qlive[r]) continue;
-      const float tot = sum[r];
-      const float inv = tot > 0.f ? 1.0f / tot : 0.f;
-      if (lane % 4 == 0 && a.lse != nullptr)
-        a.lse[((size_t)b * a.H + h) * a.Lq + qi[r]] = tot > 0.f ? (m2[r] + lg2f(tot)) * LN2 : INFINITY;
-      __nv_bfloat16 *op = a.out + (size_t)b * a.o_bs + (size_t)qi[r] * a.o_rs + h * DH + cq;
+    for (int j = 0; j < 8; ++j) {
+      if (8 * j >= n) break;
+      const float2 k2 = *reinterpret_cast<const float2 *>(kb + blk * 64 + 8 * j + cq);
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<uint32_t *>(op + 8 * j) = pack_bf16(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+      for (int r = 0; r < 2; ++r)
+        m2[r] = fmaxf(m2[r], fmaxf(fmaf(s[4 * j + 2 * r], c2, k2.x), fmaf(s[4 * j + 2 * r + 1], c2, k2.y)));
     }
-    __syncthreads();   // sQ and sP are reused by the next query tile
+  };
+  for (int blk = 0; blk < nblk; ++blk) {
+    s_block(s, blk);
+    row_max(blk);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    m2[r] = fmaxf(m2[r], __shfl_xor_sync(0xffffffffu, m2[r], 1));
+    m2[r] = fmaxf(m2[r], __shfl_xor_sync(0xffffffffu, m2[r], 2));
+    if (m2[r] == -INFINITY) m2[r] = 0.f;  // every key masked: all weights 0, output row 0
+  }
+
+  // ---- pass 2: p = 2^(x - max), row sum, dropout, bf16 P block, O += P V -------------------------------------------------
+  float sum[2] = {0.f, 0.f};
+  float o[32];
+  for (int blk = 0; blk < nblk; ++blk) {
+    const int n = block_cols(blk, NK);
+    // completes the P V chain of block blk - 1 too; every warp passed its wait for the chain of block blk - 2 before the
+    // barrier that ended block blk - 1, so this block's P buffer is free
+    s_block(s, blk);
+    uint8_t *P = sP + (blk & 1) * 8192;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      if (8 * j >= n) {   // keys past NK: zero weights (the P V chain runs over the whole block)
+        *reinterpret_cast<uint32_t *>(P + tile_off(64, rl, 8 * j + cq)) = 0u;
+        *reinterpret_cast<uint32_t *>(P + tile_off(64, rl + 8, 8 * j + cq)) = 0u;
+        continue;
+      }
+      const int col = blk * 64 + 8 * j + cq;
+      const float2 k2 = *reinterpret_cast<const float2 *>(kb + col);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float x0 = fmaf(s[4 * j + 2 * r], c2, k2.x) - m2[r], x1 = fmaf(s[4 * j + 2 * r + 1], c2, k2.y) - m2[r];
+        if (GATED && loc[r] != nullptr) {
+          if (col < a.Lk) {
+            const float *l = loc[r] + (size_t)col * 5;
+            x0 += gw[r].log2gate(__ldg(l), __ldg(l + 1), __ldg(l + 2), __ldg(l + 3), __ldg(l + 4));
+          }
+          if (col + 1 < a.Lk) {
+            const float *l = loc[r] + (size_t)(col + 1) * 5;
+            x1 += gw[r].log2gate(__ldg(l), __ldg(l + 1), __ldg(l + 2), __ldg(l + 3), __ldg(l + 4));
+          }
+        }
+        float p0 = ex2f(x0), p1 = ex2f(x1);
+        sum[r] += p0 + p1;
+        if (DROP) {
+          const uint32_t hh = drop_pair_hash(rk[r], (uint32_t)col >> 1);
+          p0 = (hh & 0xFFFFu) >= a.t16 ? p0 * a.inv_keep : 0.f;
+          p1 = (hh >> 16) >= a.t16 ? p1 * a.inv_keep : 0.f;
+        }
+        // unnormalised probabilities -> bf16 A operand; 1 / sum is applied to the fp32 output row
+        *reinterpret_cast<uint32_t *>(P + tile_off(64, rl + 8 * r, 8 * j + cq)) = pack_bf16(p0, p1);
+      }
+    }
+    fence_proxy_async_smem();
+    __syncthreads();   // the block's P is complete
+    wgmma_fence();
+    // V staged once, read MN-major; all four k16 steps (a chain cut short at the last block makes ptxas serialize it);
+    // left in flight behind the next S chain
+    mma_gc(o, aP + (blk & 1) * 8192, aV + blk * 8192, 64, blk > 0);
+    wgmma_commit();
+  }
+  wgmma_wait<0>();
+  fence_regs(o);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 1);
+    sum[r] += __shfl_xor_sync(0xffffffffu, sum[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (!qlive[r]) continue;
+    const float tot = sum[r];
+    const float inv = tot > 0.f ? 1.0f / tot : 0.f;
+    if (lane % 4 == 0 && a.lse != nullptr)
+      a.lse[((size_t)b * a.H + h) * a.Lq + qi[r]] = tot > 0.f ? (m2[r] + lg2f(tot)) * LN2 : INFINITY;
+    __nv_bfloat16 *op = a.out + (size_t)b * a.o_bs + (size_t)qi[r] * a.o_rs + h * DH + cq;
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      *reinterpret_cast<uint32_t *>(op + 8 * j) = pack_bf16(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
   }
 }
 
 template <bool GATED, bool DROP>
 int launch_fwd(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const FwdArgs &a, cudaStream_t st) {
-  const int NK64 = (a.Lk + 63) & ~63;
-  const size_t smem = 1024 + 16384 + (size_t)NK64 * 128 * 2 + (size_t)NK64 * 256 + 384 * 4 + 64;
-  constexpr size_t SMEM_MAX = 1024 + 16384 + 384 * 128 * 2 + 384 * 256 + 384 * 4 + 64;
+  const int NK = (a.Lk + 15) & ~15, NK64 = (a.Lk + 63) & ~63;
+  const size_t smem = 1024 + 8192 + (size_t)(NK + NK64) * 128 + 16384 + 384 * 4 + 8;
+  constexpr size_t SMEM_MAX = 1024 + 8192 + 384 * 128 * 2 + 16384 + 384 * 4 + 8;
   auto kern = attn_fwd_kernel<GATED, DROP>;
   static bool configured[64] = {false};
   int dev = 0;
@@ -217,7 +218,7 @@ int launch_fwd(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     configured[dev] = true;
   }
-  kern<<<a.B * a.H, 256, smem, st>>>(mq, mk, mv, a);
+  kern<<<a.B * a.H * ((a.Lq + 63) >> 6), 128, smem, st>>>(mq, mk, mv, a);
   return sv::after_launch();
 }
 

@@ -5,11 +5,10 @@
 // P is recomputed from Q, K, the gate and the saved log-sum-exp; the dropout mask is regenerated from (seed, indices);
 // no (B,H,L,T) tensor is ever stored.  Reference math: autograd of modules/layers/transformers.py:188-237 and of
 // nn.MultiheadAttention's core (transformers.py:22-24,69-74,118-120).
-// Structure (both sides): the "row" operand pair (Q,dO | K,V) is a 128-row TMA tile, each warpgroup owns 64 of its rows;
-// the "column" operand pair (K,V | Q,dO) is streamed in blocks of 64 rows through a two-deep TMA ring (the next block
-// lands while the current one is processed).  Per block: two wgmma chains give S and dP in registers (32 + 32 per
-// thread), the element-wise stage writes the bf16 dS / P tiles of the warpgroup's rows, and the output wgmma chains
-// accumulate over the blocks in registers, reading the SAME staged block MN-major.
+// Structure (both sides): the "row" operand pair (Q,dO | K,V) is a 64-row TMA tile owned by the CTA's one warpgroup; the
+// "column" operand pair (K,V | Q,dO) is streamed in blocks of 64 rows through a two-deep TMA ring.  Per block: two wgmma
+// chains give S and dP in registers (32 + 32 per thread), the element-wise stage writes the bf16 dS / P tiles, and the
+// output wgmma chains accumulate over the blocks in registers, reading the SAME staged block MN-major.
 #include "attn_common.cuh"
 #include "svgps.h"
 
@@ -33,76 +32,77 @@ struct BwdArgs {
   const unsigned long long *seed_offset;  // device counter added to the seed at run time (or null)
 };
 
-// acc[64 rows x 64] (+)= A[64 rows x 64] . B[64 x 64]^T, both K-major 128-byte-swizzle tiles
-__device__ __forceinline__ void mma_kk(float (&d)[32], uint32_t aA, uint32_t aB) {
-#pragma unroll
-  for (int ks = 0; ks < DH / 16; ++ks) wgmma_n64<0, 0>(d, desc_sw128(aA + ks * 32, 16), desc_sw128(aB + ks * 32, 16), ks > 0);
-}
-// acc (+)= G[64 rows x 64 block columns] (canonical no-swizzle K-major) . C[64 block rows x 64] (read MN-major)
-__device__ __forceinline__ void mma_gc(float (&d)[32], uint32_t aG, uint32_t aC, bool accumulate) {
-#pragma unroll
-  for (int ks = 0; ks < 4; ++ks)
-    wgmma_n64<0, 1>(d, desc_noswz(aG + ks * 4096, 2048, 128), desc_sw128(aC + ks * 2048, 8192), (accumulate || ks > 0) ? 1u : 0u);
-}
 // 64 columns of a row from the accumulator fragment (row r_lo + 8 r) -> bf16 row of `dst`
 __device__ __forceinline__ void store_row_frag(const float (&d)[32], int r, __nv_bfloat16 *dst, int cq) {
 #pragma unroll
   for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t *>(dst + 8 * j + cq) = pack_bf16(d[4 * j + 2 * r], d[4 * j + 2 * r + 1]);
 }
 
+constexpr int BWD_STAGES = 2;   // column-block ring: block j + 1 lands while block j is processed
+
+template <int SIDE>
+constexpr size_t bwd_smem_bytes(int NC, bool gated) {
+  return 1024 + 16384 + (size_t)BWD_STAGES * 16384 + (SIDE == 1 ? 16384 : 8192) +
+         (size_t)(SIDE == 0 ? NC : (gated ? 9 : 3) * NC) * 4 + 8 * (BWD_STAGES + 1);
+}
+
+// One CTA = one warpgroup = one unit (scene, head, 64 rows of the row operand), CTAs ordered by (scene, head) first so
+// that the units of one head share its column operand in L2.  Per column block: S and dP wgmma chains; once they are
+// complete the staging buffer of the block two ahead is free (its output chain, issued one block earlier, completed with
+// them) and the TMA load of the next block is issued; the element-wise stage writes the bf16 dS (and P) tile; the output
+// chains are issued and left in flight behind the next block's S / dP chains.
 template <int SIDE, bool GATED, bool DROP>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(128, 3)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__ CUtensorMap mR2,
                 const __grid_constant__ CUtensorMap mC1, const __grid_constant__ CUtensorMap mC2, const BwdArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int Lr = SIDE == 0 ? a.Lq : a.Lk;    // rows of the tiles
   const int Lc = SIDE == 0 ? a.Lk : a.Lq;    // columns swept in blocks of 64
-  const int NC = (Lc + 63) & ~63;
-  uint8_t *sR1 = smem;                       // [128][64] sw128   Q  | K
-  uint8_t *sR2 = sR1 + 16384;                // [128][64] sw128   dO | V
-  uint8_t *sC = sR2 + 16384;                 // 2 buffers x { [64][64] sw128 K | Q block, [64][64] sw128 V | dO block }
-  uint8_t *sG1 = sC + 2 * 16384;             // [8][128][8] K-major   scale * dS (^T)
-  uint8_t *sG2 = sG1 + 16384;                // [8][128][8] K-major   dropped P^T (SIDE 1)
-  float *vec = reinterpret_cast<float *>(sG2 + (SIDE == 1 ? 16384 : 0));
+  const int NC = (Lc + 15) & ~15;            // columns rounded to the 16-column granule
+  uint8_t *sR1 = smem;                       // [64][64] sw128   Q  | K
+  uint8_t *sR2 = sR1 + 8192;                 // [64][64] sw128   dO | V
+  uint8_t *sC = sR2 + 8192;                  // BWD_STAGES x { [64][64] sw128 K | Q block, [64][64] sw128 V | dO block }
+  uint8_t *sG1 = sC + BWD_STAGES * 16384;    // [8][64][8] K-major   scale * dS (^T)
+  uint8_t *sG2 = sG1 + 8192;                 // [8][64][8] K-major   dropped P^T (SIDE 1)
+  float *vec = reinterpret_cast<float *>(sG2 + (SIDE == 1 ? 8192 : 0));
   // SIDE 0: vec = kb[NC]      SIDE 1: vec = lse2[NC] | Dv[NC] | rk[NC] | W[NC][6] (GATED)
   float *kb = vec;
   float *lse2s = vec, *Dv = vec + NC;
   uint32_t *rks = reinterpret_cast<uint32_t *>(vec + 2 * NC);
   float *Ws = vec + 3 * NC;
-  // barriers 0,1: column block landed in buffer 0 / 1, 2: row tile landed
-  uint64_t *bars = reinterpret_cast<uint64_t *>(vec + (SIDE == 0 ? NC : 9 * NC));
+  // barriers [0, BWD_STAGES): column block landed in that buffer, BWD_STAGES: row tile landed
+  uint64_t *bars = reinterpret_cast<uint64_t *>(vec + (SIDE == 0 ? NC : (GATED ? 9 : 3) * NC));
 
-  const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127, w = t >> 5, lane = tid & 31;
-  const int rl = wg * 64 + w * 16 + (lane >> 2);   // this thread's first row in the tile (second: rl + 8)
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
+  const int rl = w * 16 + (lane >> 2);             // this thread's first row in the tile (second: rl + 8)
   const int cq = 2 * (lane & 3);                   // its first column in every 8-column group
-  const int b = blockIdx.x / a.H, h = blockIdx.x % a.H;
+  const int ntile = (Lr + 63) >> 6;
+  const int bh = blockIdx.x / ntile, r0 = (blockIdx.x % ntile) * 64;
+  const int b = bh / a.H, h = bh % a.H;
   const int E = a.H * DH;
-  const int nblk = NC >> 6;
-  const int ntile = (Lr + 127) >> 7;
-  // work item i = (row tile i / nblk, column block i % nblk) -> staging buffer i & 1
-  auto load_cblock = [&](int i) {
-    const int cb = i % nblk, buf = i & 1;
-    mbar_expect_tx(&bars[buf], 2 * rows_bytes(cb * 64, 4, Lc));
-    tma_rows(sC + buf * 16384, &mC1, h, cb * 64, 4, Lc, b, &bars[buf]);
-    tma_rows(sC + buf * 16384 + 8192, &mC2, h, cb * 64, 4, Lc, b, &bars[buf]);
+  const int nblk = (NC + 63) >> 6;
+  auto load_cblock = [&](int blk) {
+    const int buf = blk % BWD_STAGES;
+    mbar_expect_tx(&bars[buf], 2 * rows_bytes(blk * 64, 4, Lc));
+    tma_rows(sC + buf * 16384, &mC1, h, blk * 64, 4, Lc, b, &bars[buf]);
+    tma_rows(sC + buf * 16384 + 8192, &mC2, h, blk * 64, 4, Lc, b, &bars[buf]);
   };
 
   if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    mbar_init(&bars[2], 1);
+#pragma unroll
+    for (int i = 0; i <= BWD_STAGES; ++i) mbar_init(&bars[i], 1);
     mbar_fence_init();
     tma_prefetch_desc(&mR1);
     tma_prefetch_desc(&mR2);
     tma_prefetch_desc(&mC1);
     tma_prefetch_desc(&mC2);
   }
-  // operand rows past the sequence ends are never written by TMA: start from zeros so that they only ever hold finite
-  // values (their products are multiplied by exact zeros of P / dS)
-  for (int i = tid; i < 4 * 16384 / 16; i += 256) reinterpret_cast<uint4 *>(smem)[i] = make_uint4(0, 0, 0, 0);
+  // row-tile rows past the sequence end are never written by TMA: start from zeros so that they only ever hold finite
+  // values.  Column-block rows past the last box only reach S / dP columns the element-wise stage never reads.
+  for (int i = tid; i < 16384 / 16; i += 128) reinterpret_cast<uint4 *>(smem)[i] = make_uint4(0, 0, 0, 0);
   // per-column vectors
-  for (int c = tid; c < NC; c += 256) {
+  for (int c = tid; c < NC; c += 128) {
     if (SIDE == 0) {
       kb[c] = (c < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + c])) ? 0.f : -INFINITY;
     } else {
@@ -120,183 +120,178 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
   }
   fence_proxy_async_smem();
   __syncthreads();
-  if (tid == 0) load_cblock(0);
+  if (tid == 0) {
+    mbar_expect_tx(&bars[BWD_STAGES], 2 * rows_bytes(r0, 4, Lr));
+    tma_rows(sR1, &mR1, h, r0, 4, Lr, b, &bars[BWD_STAGES]);
+    tma_rows(sR2, &mR2, h, r0, 4, Lr, b, &bars[BWD_STAGES]);
+    for (int i = 0; i < BWD_STAGES - 1 && i < nblk; ++i) load_cblock(i);
+  }
   const float c2 = a.scale * LOG2E;
-  const uint32_t aR1 = smem_u32(sR1) + wg * 8192, aR2 = smem_u32(sR2) + wg * 8192;
-  const uint32_t aG1 = smem_u32(sG1) + wg * 1024, aG2 = smem_u32(sG2) + wg * 1024;
-  uint32_t ph_r = 0;
-  int item = 0;
+  const uint32_t aR1 = smem_u32(sR1), aR2 = smem_u32(sR2);
+  const uint32_t aG1 = smem_u32(sG1), aG2 = smem_u32(sG2);
 
-  for (int tile = 0; tile < ntile; ++tile) {
-    const int r0 = tile * 128;
-    if (tid == 0) {
-      mbar_expect_tx(&bars[2], 2 * rows_bytes(r0, 8, Lr));
-      tma_rows(sR1, &mR1, h, r0, 8, Lr, b, &bars[2]);
-      tma_rows(sR2, &mR2, h, r0, 8, Lr, b, &bars[2]);
+  // ---- per-row state (rows rl and rl + 8 of the tile) ----------------------------------------------------------------
+  int ri[2];
+  bool rlive[2], klive[2];
+  float lse2[2] = {INFINITY, INFINITY}, D[2] = {0.f, 0.f};   // SIDE 0
+  GateW gw[2];
+  const float *loc[2] = {nullptr, nullptr};
+  uint32_t rk[2] = {0u, 0u};
+  float gg[2][6];                                            // SIDE 0, GATED: d/d(bias, w1..w5) partial sums
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) gg[r][k] = 0.f;
+    ri[r] = r0 + rl + 8 * r;
+    rlive[r] = ri[r] < Lr;
+    klive[r] = false;
+    if (SIDE == 0) {
+      if (rlive[r]) {
+        const size_t rr = ((size_t)b * a.H + h) * a.Lq + ri[r];
+        lse2[r] = a.lse[rr] * LOG2E;
+        const uint4 *po = reinterpret_cast<const uint4 *>(a.o + ((size_t)b * a.Lq + ri[r]) * E + h * DH);
+        const uint4 *pd = reinterpret_cast<const uint4 *>(a.d_o + ((size_t)b * a.Lq + ri[r]) * E + h * DH);
+        float dd = 0.f;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          const uint4 x = __ldg(po + c), y = __ldg(pd + c);
+          const __nv_bfloat162 *xa = reinterpret_cast<const __nv_bfloat162 *>(&x);
+          const __nv_bfloat162 *ya = reinterpret_cast<const __nv_bfloat162 *>(&y);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float2 u = __bfloat1622float2(xa[i]), v = __bfloat1622float2(ya[i]);
+            dd = fmaf(u.x, v.x, fmaf(u.y, v.y, dd));
+          }
+        }
+        D[r] = dd;
+        if ((lane & 3) == 0) a.dvec[rr] = dd;
+        if (GATED) {
+          gw[r].load(a.sw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6);
+          loc[r] = a.locs + ((size_t)b * a.Lq + ri[r]) * (size_t)a.Lk * 5;
+        }
+        if (DROP) rk[r] = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), rr);
+      }
+    } else {
+      klive[r] = rlive[r] && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + ri[r]]);
     }
-    // ---- per-row state (rows rl and rl + 8 of the tile) ----------------------------------------------------------------
-    int ri[2];
-    bool rlive[2], klive[2];
-    float lse2[2] = {INFINITY, INFINITY}, D[2] = {0.f, 0.f};   // SIDE 0
-    GateW gw[2];
-    const float *loc[2] = {nullptr, nullptr};
-    uint32_t rk[2] = {0u, 0u};
-    float gg[2][6];                                            // SIDE 0, GATED: d/d(bias, w1..w5) partial sums
+  }
+  mbar_wait(&bars[BWD_STAGES], 0);
+
+  float o1[32], o2[32];
+  for (int blk = 0; blk < nblk; ++blk) {
+    const int buf = blk % BWD_STAGES, n = block_cols(blk, NC);
+    mbar_wait(&bars[buf], (uint32_t)(blk / BWD_STAGES) & 1u);
+    const uint32_t aC1 = smem_u32(sC) + buf * 16384, aC2 = aC1 + 8192;
+    // ---- S_blk, dP_blk (queued behind the previous block's output chains) ---------------------------------------------
+    float sa[32], dp[32];
+    wgmma_fence();
+    mma_kk(sa, aR1, aC1);
+    mma_kk(dp, aR2, aC2);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(sa);
+    fence_regs(dp);
+    // every warp's chains are complete: the buffer of block blk - 1 and the dS / P tiles are free
+    __syncthreads();
+    if (tid == 0 && blk + BWD_STAGES - 1 < nblk) load_cblock(blk + BWD_STAGES - 1);
+
+    // ---- element-wise stage over this thread's fragment: rows rl + 8 r, columns 8 j + cq + e of the block ------------
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
+    for (int j = 0; j < 8; ++j) {
+      if (8 * j >= n) break;
+      const int cl = 8 * j + cq;             // column inside the block
+      const int c0 = blk * 64 + cl;          // global column (key for SIDE 0, query for SIDE 1)
 #pragma unroll
-      for (int k = 0; k < 6; ++k) gg[r][k] = 0.f;
-      ri[r] = r0 + rl + 8 * r;
-      rlive[r] = ri[r] < Lr;
-      klive[r] = false;
-      if (SIDE == 0) {
-        if (rlive[r]) {
-          const size_t rr = ((size_t)b * a.H + h) * a.Lq + ri[r];
-          lse2[r] = a.lse[rr] * LOG2E;
-          const uint4 *po = reinterpret_cast<const uint4 *>(a.o + ((size_t)b * a.Lq + ri[r]) * E + h * DH);
-          const uint4 *pd = reinterpret_cast<const uint4 *>(a.d_o + ((size_t)b * a.Lq + ri[r]) * E + h * DH);
-          float dd = 0.f;
+      for (int r = 0; r < 2; ++r) {
+        float ds[2], pd[2];
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const uint4 x = __ldg(po + c), y = __ldg(pd + c);
-            const __nv_bfloat162 *xa = reinterpret_cast<const __nv_bfloat162 *>(&x);
-            const __nv_bfloat162 *ya = reinterpret_cast<const __nv_bfloat162 *>(&y);
+        for (int e = 0; e < 2; ++e) {
+          const int c = c0 + e;
+          const float sv = sa[4 * j + 2 * r + e];
+          float dpi = dp[4 * j + 2 * r + e];
+          float p, m = 1.f;
+          if (SIDE == 0) {
+            float gli = 0.f;
+            float l5[5];
+            const bool have = GATED && loc[r] != nullptr && c < a.Lk;
+            if (have) {
+              const float *lp = loc[r] + (size_t)c * 5;
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 u = __bfloat1622float2(xa[i]), v = __bfloat1622float2(ya[i]);
-              dd = fmaf(u.x, v.x, fmaf(u.y, v.y, dd));
+              for (int k = 0; k < 5; ++k) l5[k] = __ldg(lp + k);
+              gli = gw[r].log2gate(l5[0], l5[1], l5[2], l5[3], l5[4]);
             }
-          }
-          D[r] = dd;
-          if ((lane & 3) == 0) a.dvec[rr] = dd;
-          if (GATED) {
-            gw[r].load(a.sw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6);
-            loc[r] = a.locs + ((size_t)b * a.Lq + ri[r]) * (size_t)a.Lk * 5;
-          }
-          if (DROP) rk[r] = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), rr);
-        }
-      } else {
-        klive[r] = rlive[r] && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + ri[r]]);
-      }
-    }
-    mbar_wait(&bars[2], ph_r);
-    ph_r ^= 1u;
-
-    float o1[32], o2[32];
-    for (int blk = 0; blk < nblk; ++blk, ++item) {
-      const int buf = item & 1;
-      // the other buffer was last read by the previous item, which every thread has finished (barrier at its end)
-      if (tid == 0 && item + 1 < ntile * nblk) load_cblock(item + 1);
-      mbar_wait(&bars[buf], (uint32_t)(item >> 1) & 1u);
-      const uint32_t aC1 = smem_u32(sC) + buf * 16384, aC2 = aC1 + 8192;
-      // ---- S_blk, dP_blk -----------------------------------------------------------------------------------------------
-      float sa[32], dp[32];
-      wgmma_fence();
-      mma_kk(sa, aR1, aC1);
-      mma_kk(dp, aR2, aC2);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(sa);
-      fence_regs(dp);
-
-      // ---- element-wise stage over this thread's fragment: rows rl + 8 r, columns 8 j + cq + e of the block ----------
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const int cl = 8 * j + cq;             // column inside the block
-        const int c0 = blk * 64 + cl;          // global column (key for SIDE 0, query for SIDE 1)
-#pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          float ds[2], pd[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = c0 + e;
-            const float sv = sa[4 * j + 2 * r + e];
-            float dpi = dp[4 * j + 2 * r + e];
-            float p, m = 1.f;
-            if (SIDE == 0) {
-              float gli = 0.f;
-              float l5[5];
-              const bool have = GATED && loc[r] != nullptr && c < a.Lk;
-              if (have) {
-                const float *lp = loc[r] + (size_t)c * 5;
-#pragma unroll
-                for (int k = 0; k < 5; ++k) l5[k] = __ldg(lp + k);
-                gli = gw[r].log2gate(l5[0], l5[1], l5[2], l5[3], l5[4]);
-              }
-              p = ex2f(fmaf(sv, c2, kb[c]) - lse2[r] + gli);
-              if (DROP) {
-                const uint32_t hh = drop_pair_hash(rk[r], (uint32_t)c >> 1);
-                m = drop_keep(hh, (uint32_t)c, a.t16) ? a.inv_keep : 0.f;
-                dpi *= m;
-              }
-              const float dsi = p * (dpi - D[r]);
-              if (GATED && have && gli > LOG2_CLAMP) {                 // clamp(sigmoid, 1e-6) inactive
-                const float dz = dsi * (1.0f - ex2f(gli));            // d log(sigmoid(z)) / dz = 1 - sigmoid(z)
-                gg[r][0] += dz;
-#pragma unroll
-                for (int k = 0; k < 5; ++k) gg[r][1 + k] = fmaf(dz, l5[k], gg[r][1 + k]);
-              }
-              ds[e] = dsi * a.scale;
-              pd[e] = p * m;
-            } else {
-              float gl = 0.f;
-              if (GATED && klive[r] && c < a.Lq) {
-                const float *wv = Ws + c * 6;
-                const GateW g{wv[0], wv[1], wv[2], wv[3], wv[4], wv[5]};
-                const float *l = a.locs + (((size_t)b * a.Lq + c) * a.Lk + ri[r]) * 5;
-                gl = g.log2gate(__ldg(l), __ldg(l + 1), __ldg(l + 2), __ldg(l + 3), __ldg(l + 4));
-              }
-              p = klive[r] ? ex2f(fmaf(sv, c2, -lse2s[c]) + gl) : 0.f;
-              if (DROP) {
-                const uint32_t hh = drop_pair_hash(rks[c], (uint32_t)ri[r] >> 1);
-                m = drop_keep(hh, (uint32_t)ri[r], a.t16) ? a.inv_keep : 0.f;
-                dpi *= m;
-              }
-              ds[e] = p * (dpi - Dv[c]) * a.scale;
-              pd[e] = p * m;
+            p = ex2f(fmaf(sv, c2, kb[c]) - lse2[r] + gli);
+            if (DROP) {
+              const uint32_t hh = drop_pair_hash(rk[r], (uint32_t)c >> 1);
+              m = drop_keep(hh, (uint32_t)c, a.t16) ? a.inv_keep : 0.f;
+              dpi *= m;
             }
+            const float dsi = p * (dpi - D[r]);
+            if (GATED && have && gli > LOG2_CLAMP) {                 // clamp(sigmoid, 1e-6) inactive
+              const float dz = dsi * (1.0f - ex2f(gli));            // d log(sigmoid(z)) / dz = 1 - sigmoid(z)
+              gg[r][0] += dz;
+#pragma unroll
+              for (int k = 0; k < 5; ++k) gg[r][1 + k] = fmaf(dz, l5[k], gg[r][1 + k]);
+            }
+            ds[e] = dsi * a.scale;
+            pd[e] = p * m;
+          } else {
+            float gl = 0.f;
+            if (GATED && klive[r] && c < a.Lq) {
+              const float *wv = Ws + c * 6;
+              const GateW g{wv[0], wv[1], wv[2], wv[3], wv[4], wv[5]};
+              const float *l = a.locs + (((size_t)b * a.Lq + c) * a.Lk + ri[r]) * 5;
+              gl = g.log2gate(__ldg(l), __ldg(l + 1), __ldg(l + 2), __ldg(l + 3), __ldg(l + 4));
+            }
+            p = klive[r] ? ex2f(fmaf(sv, c2, -lse2s[c]) + gl) : 0.f;
+            if (DROP) {
+              const uint32_t hh = drop_pair_hash(rks[c], (uint32_t)ri[r] >> 1);
+              m = drop_keep(hh, (uint32_t)ri[r], a.t16) ? a.inv_keep : 0.f;
+              dpi *= m;
+            }
+            ds[e] = p * (dpi - Dv[c]) * a.scale;
+            pd[e] = p * m;
           }
-          const uint32_t off = tile_off(128, rl + 8 * r, cl);
-          *reinterpret_cast<uint32_t *>(sG1 + off) = pack_bf16(ds[0], ds[1]);
-          if (SIDE == 1) *reinterpret_cast<uint32_t *>(sG2 + off) = pack_bf16(pd[0], pd[1]);
         }
+        const uint32_t off = tile_off(64, rl + 8 * r, cl);
+        *reinterpret_cast<uint32_t *>(sG1 + off) = pack_bf16(ds[0], ds[1]);
+        if (SIDE == 1) *reinterpret_cast<uint32_t *>(sG2 + off) = pack_bf16(pd[0], pd[1]);
       }
-      fence_proxy_async_smem();
-      wg_sync(1 + wg);   // this warpgroup's rows of dS (and P) are complete
-
-      // ---- accumulate the outputs over this block's columns (column operand read MN-major) -------------------------------
-      wgmma_fence();
-      mma_gc(o1, aG1, aC1, blk > 0);
-      if (SIDE == 1) mma_gc(o2, aG2, aC2, blk > 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(o1);
-      if (SIDE == 1) fence_regs(o2);
-      __syncthreads();   // both warpgroups are done with this column buffer and with sG1 / sG2
     }
+    fence_proxy_async_smem();
+    __syncthreads();   // the tile's dS (and P) are complete
 
-    // ---- epilogue ----------------------------------------------------------------------------------------------------------
+    // ---- accumulate the outputs over this block's columns (column operand read MN-major), left in flight ---------------
+    wgmma_fence();
+    mma_gc(o1, aG1, aC1, n, blk > 0);
+    if (SIDE == 1) mma_gc(o2, aG2, aC2, n, blk > 0);
+    wgmma_commit();
+  }
+  wgmma_wait<0>();
+  fence_regs(o1);
+  if (SIDE == 1) fence_regs(o2);
+
+  // ---- epilogue ----------------------------------------------------------------------------------------------------------
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      if (SIDE == 0 && GATED) {
+  for (int r = 0; r < 2; ++r) {
+    if (SIDE == 0 && GATED) {
 #pragma unroll
-        for (int k = 0; k < 6; ++k) {
-          gg[r][k] += __shfl_xor_sync(0xffffffffu, gg[r][k], 1);
-          gg[r][k] += __shfl_xor_sync(0xffffffffu, gg[r][k], 2);
-        }
+      for (int k = 0; k < 6; ++k) {
+        gg[r][k] += __shfl_xor_sync(0xffffffffu, gg[r][k], 1);
+        gg[r][k] += __shfl_xor_sync(0xffffffffu, gg[r][k], 2);
       }
-      if (!rlive[r]) continue;
-      if (SIDE == 0) {
-        store_row_frag(o1, r, a.dq + ((size_t)b * a.Lq + ri[r]) * a.d_rs + h * DH, cq);
-        if (GATED && (lane & 3) == 0 && a.dsw != nullptr) {
-          float *g = a.dsw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6;
+    }
+    if (!rlive[r]) continue;
+    if (SIDE == 0) {
+      store_row_frag(o1, r, a.dq + ((size_t)b * a.Lq + ri[r]) * a.d_rs + h * DH, cq);
+      if (GATED && (lane & 3) == 0 && a.dsw != nullptr) {
+        float *g = a.dsw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6;
 #pragma unroll
-          for (int k = 0; k < 6; ++k) g[k] = gg[r][k];
-        }
-      } else {
-        store_row_frag(o1, r, a.dk + ((size_t)b * a.Lk + ri[r]) * a.d_rs + h * DH, cq);
-        store_row_frag(o2, r, a.dv + ((size_t)b * a.Lk + ri[r]) * a.d_rs + h * DH, cq);
+        for (int k = 0; k < 6; ++k) g[k] = gg[r][k];
       }
+    } else {
+      store_row_frag(o1, r, a.dk + ((size_t)b * a.Lk + ri[r]) * a.d_rs + h * DH, cq);
+      store_row_frag(o2, r, a.dv + ((size_t)b * a.Lk + ri[r]) * a.d_rs + h * DH, cq);
     }
   }
 }
@@ -304,10 +299,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
 template <int SIDE, bool GATED, bool DROP>
 int launch_side(const CUtensorMap &r1, const CUtensorMap &r2, const CUtensorMap &c1, const CUtensorMap &c2,
                 const BwdArgs &a, cudaStream_t st) {
-  const int Lc = SIDE == 0 ? a.Lk : a.Lq;
-  const int NC = (Lc + 63) & ~63;
-  const size_t smem = 1024 + 32768 + 32768 + (SIDE == 1 ? 32768 : 16384) + (size_t)(SIDE == 0 ? NC : 9 * NC) * 4 + 64;
-  constexpr size_t SMEM_MAX = 1024 + 32768 + 32768 + 32768 + 9 * 384 * 4 + 64;
+  const int Lr = SIDE == 0 ? a.Lq : a.Lk, Lc = SIDE == 0 ? a.Lk : a.Lq;
+  const size_t smem = bwd_smem_bytes<SIDE>((Lc + 15) & ~15, GATED);
+  constexpr size_t SMEM_MAX = bwd_smem_bytes<SIDE>(384, GATED);
   auto kern = attn_bwd_kernel<SIDE, GATED, DROP>;
   static bool configured[64] = {false};
   int dev = 0;
@@ -319,7 +313,7 @@ int launch_side(const CUtensorMap &r1, const CUtensorMap &r2, const CUtensorMap 
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
     configured[dev] = true;
   }
-  kern<<<a.B * a.H, 256, smem, st>>>(r1, r2, c1, c2, a);
+  kern<<<a.B * a.H * ((Lr + 63) >> 6), 128, smem, st>>>(r1, r2, c1, c2, a);
   return sv::after_launch();
 }
 

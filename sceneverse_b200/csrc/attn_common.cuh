@@ -7,8 +7,14 @@
 //   * a K-major operand (contraction over the 64 head dims):   sm90::desc_sw128(addr, 16), K step = +32 B;
 //   * an MN-major B operand (contraction over the ROWS, N = 64 head dims, e.g. P.V, dS.K): sm90::desc_sw128 read with
 //     the wgmma transpose flag, K step of 16 rows = +2048 B — no transposed copy is ever built.
-// Thread-written A operands (P, dS, P^T, dS^T) use the canonical no-swizzle K-major layout tile[K/8][128][8]
+// Thread-written A operands (P, dS, P^T, dS^T) use the canonical no-swizzle K-major layout tile[K/8][64][8]
 // (sm90::tile_off, sm90::desc_noswz).
+//
+// Work unit: one (scene, head, 64-row tile) per CTA of one warpgroup; several CTAs share an SM and run independently, so
+// one unit's element-wise stage overlaps another's wgmma chains.  The column dimension is swept in blocks of 64; the
+// element-wise work and the backward's output chains of the last block stop at the column count rounded up to 16 (the
+// TMA box and the k16 step).  Every output element keeps the chain of k16 steps it had with whole 64-column blocks: the
+// skipped steps only ever added products with exact zeros.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -75,6 +81,29 @@ struct GateW {
     return fmaxf(-lg2f(1.0f + t), LOG2_CLAMP);
   }
 };
+
+// ---- wgmma chains of one 64-row unit -----------------------------------------------------------------------------------
+// width of column block `blk` of a sweep over `n16` columns (a multiple of 16): 64, the last one 16, 32, 48 or 64
+__device__ __forceinline__ int block_cols(int blk, int n16) {
+  const int rest = n16 - blk * 64;
+  return rest < 64 ? rest : 64;
+}
+// acc[64 rows x 64] = A[64 rows x 64] . B[64 x 64]^T, both K-major 128-byte-swizzle tiles (contraction over the head dims).
+// A last block narrower than 64 is still computed whole: a narrower wgmma form for it makes ptxas serialize the chains,
+// and its columns past the block width (products with stale staging rows) are never read.
+__device__ __forceinline__ void mma_kk(float (&d)[32], uint32_t aA, uint32_t aB) {
+#pragma unroll
+  for (int ks = 0; ks < DH / 16; ++ks) wgmma_n64<0, 0>(d, desc_sw128(aA + ks * 32, 16), desc_sw128(aB + ks * 32, 16), ks > 0);
+}
+// acc[64 rows x 64] (+)= G[64 rows x n] . C[n x 64]: G thread-written in the no-swizzle K-major tile[8][64][8], C a staged
+// [n][64] 128-byte-swizzle block read MN-major (contraction over its rows); n / 16 k16 steps
+__device__ __forceinline__ void mma_gc(float (&d)[32], uint32_t aG, uint32_t aC, int n, bool accumulate) {
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks)
+    if (ks * 16 < n)
+      wgmma_n64<0, 1>(d, desc_noswz(aG + ks * 2048, 1024, 128), desc_sw128(aC + ks * 2048, 8192),
+                      (accumulate || ks > 0) ? 1u : 0u);
+}
 
 // ---- dropout mask ----------------------------------------------------------------------------------------------------------
 // keep(b, h, i, j) is a pure function of (seed, b, h, i, j): one 64-bit mix per (scene, head, query) row gives a 32-bit

@@ -1,4 +1,5 @@
-"""Forward+backward timing of the native attention kernels against SDPA at the GPS training shapes (B = 64 scenes)."""
+"""Forward+backward timing of the native attention kernels at the GPS training shapes (B = 64 scenes): the four attention
+configurations of the pre-training step (each runs in four layers), then plain shapes against SDPA."""
 import os, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -16,6 +17,23 @@ def t(fn, n=20):
 g = torch.Generator(device="cuda").manual_seed(0)
 def rnd(*s): return torch.randn(*s, device="cuda", generator=g)
 res = {}
+# (name, L, key-padding mask, spatial gate, dropout): BERT over scene captions and over utterances, the joint
+# object-language self-attention, the gated spatial self-attention of the object encoder
+STEP = [("bert300", 300, True, False, 0.1), ("bert50", 50, True, False, 0.1), ("joint130", 130, False, False, 0.1),
+        ("spatial80", 80, True, True, 0.0)]
+for name, L, masked, gated, p in STEP:
+    q, k, v, go = (rnd(B, L, E).bfloat16() for _ in range(4))
+    kw = {}
+    if masked:
+        lens = torch.randint(1, L + 1, (B,), device="cuda", generator=g)
+        kw["key_padding_mask"] = torch.arange(L, device="cuda")[None] >= lens[:, None]
+    bkw = dict(kw, dropout_p=p, seed=5)
+    if gated:
+        bkw.update(spatial_w=rnd(B, L, H * 6), pairwise_locs=ops.calc_pairwise_locs(rnd(B, L, 3), None))
+    fkw = dict(bkw, spatial_heads=H) if gated else bkw
+    res[f"{name}_fwd"] = t(lambda: native.attention(q, k, v, H, return_lse=True, **fkw), n=100)
+    out, lse = native.attention(q, k, v, H, return_lse=True, **fkw)
+    res[f"{name}_bwd"] = t(lambda: native.attention_backward(q, k, v, out, go, lse, H, **bkw), n=100)
 for name, Lq, Lk in [("joint130", 130, 130), ("self80", 80, 80), ("cross80x50", 80, 50)]:
     q = rnd(B, Lq, E).bfloat16(); k = rnd(B, Lk, E).bfloat16(); v = rnd(B, Lk, E).bfloat16(); go = rnd(B, Lq, E).bfloat16()
     for p in (0.0, 0.1):
