@@ -181,6 +181,25 @@ class PointNetPP(nn.Module):
             self._packed_key = key
         return self._packed
 
+    @torch.no_grad()
+    def refresh_pack_(self):
+        """Re-pack the current weights INTO the existing packed images (a captured CUDA graph holds their addresses and the
+        host check of _pack never runs during replays).  Nothing to do if the fused path never packed."""
+        old = self._packed
+        if old is None:
+            return
+        self._packed = None
+        new = self._pack()
+        pairs = [(old["sa1"], new["sa1"]), (old["sa2"], new["sa2"])]
+        pairs += [(a, b) for (oa, ob), (na, nb) in zip(old["sa3"] + [old["fc"]], new["sa3"] + [new["fc"]])
+                  for a, b in ((oa, na), (ob, nb))]
+        for dst, src in pairs:
+            if dst.shape != src.shape or dst.dtype != src.dtype:
+                raise RuntimeError("PointNet++ packed weights cannot be refreshed in place: their layout changed")
+            if dst.data_ptr() != src.data_ptr():       # the fp32 fc bias is the parameter itself: already current
+                dst.copy_(src)
+        self._packed = old          # _pack() left the key of the current weights
+
     # -------------------------------------------------------------- forward
     def forward(self, features):
         """@param features: (B*N_objects, N_points, 3 + C)  ->  (B*N_objects, D)"""

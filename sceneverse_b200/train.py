@@ -27,6 +27,10 @@ class StepModule(nn.Module):
         c = M.to_cfg(cfg)
         self.loss = L.Loss(c.model.loss_list, c.model.vis_loss_list, num_gpu=c.num_gpu,
                            emulate_dist=bool(c.get("emulate_dist", False)), task=c.get("task"))
+        # the reference's optimizer groups (get_opt_params before anything is frozen here) + the loss group: the index space
+        # of a checkpoint's optimizer state
+        self.opt_order = [list(g['params']) for g in self.model.get_opt_params()]
+        self.opt_order.append([p for p in self.loss.parameters() if p.requires_grad])
         for n, p in self.model.named_parameters():
             if n.startswith(STATIC_UNUSED):
                 p.requires_grad = False
@@ -149,7 +153,10 @@ class PretrainStep:
             self.use_ddp = False
         warm = self.cfg.solver.sched.args.warmup_steps * self.cfg.num_gpu
         mr = self.cfg.solver.sched.args.get("minimum_ratio", 1e-5)
-        self._lr_lambda = lambda s: M.warmup_cosine(s, warm, total_steps, minimum_ratio=mr)
+        self.total_steps = total_steps         # read at every evaluation: a loaded checkpoint restores it
+        self._lr_lambda = lambda s: M.warmup_cosine(s, warm, self.total_steps, minimum_ratio=mr)
+        self._pending_state = None             # a checkpoint loaded before the first graph-mode step
+        self._capture_calls = None             # ops._dropout_calls when the replayed graph was captured
         if self.graph_mode:
             # capturable AdamW reads lr from a device tensor; the warm-up/cosine schedule fills it from the host per step
             self._base_lrs = [float(g.get('lr', self.cfg.solver.lr)) for g in groups]
@@ -185,6 +192,155 @@ class PretrainStep:
             raise RuntimeError("PretrainStep was built without train_eval: there are no logs")
         return self.train_log.read()
 
+    # ---- checkpoints ---------------------------------------------------------------------------------------------------
+    def state_dict(self):
+        """Everything a resumed run needs, on the host, independent of the flat layout: `model` / `loss` (state_dicts with
+        the reference's keys), `optimizer` (torch AdamW.state_dict() form, parameter indices in get_opt_params() order, loss
+        group last), `scheduler` (LambdaLR form), `random_states` (this rank's generators) and `native` (global_step,
+        total_steps, the device dropout counter, the in-kernel dropout seed position, the probed unused parameters)."""
+        if self._pending_state is not None:          # loaded, not applied yet: that state is this step's state
+            return self._pending_state
+        from . import checkpoint as C
+        flat = self._flat_state()
+        if flat is not None:
+            step = int(flat.step_t.item())
+            host = {name: getattr(flat, name).cpu() for name in ("exp_avg", "exp_avg_sq")}
+
+            def moments(p):
+                o, n = flat.offsets[id(p)], p.numel()
+                return step, host["exp_avg"][o:o + n].view(p.shape).clone(), host["exp_avg_sq"][o:o + n].view(p.shape).clone()
+        else:
+            def moments(p):
+                st = self.optimizer.state.get(p)
+                if not st:
+                    return None
+                return float(st["step"]), C.to_cpu(st["exp_avg"]), C.to_cpu(st["exp_avg_sq"])
+        base = self._base_lrs if self.scheduler is None else self.scheduler.base_lrs
+        optim = C.export_adamw(self.module.opt_order, self.optimizer.param_groups, self._lrs(), base, moments)
+        sched = self.scheduler.state_dict() if self.scheduler is not None else \
+            C.lambda_lr_state(self._base_lrs, self._sched_step, self._lrs())
+        counter = getattr(self, "_step_counter", None)
+        return {"model": C.to_cpu(self.module.model.state_dict()), "loss": C.to_cpu(self.module.loss.state_dict()),
+                "optimizer": optim, "scheduler": sched, "random_states": C.rng_state(),
+                "native": {"global_step": self.global_step, "total_steps": self.total_steps,
+                           "dropout_counter": int(counter.item()) if counter is not None else None,
+                           "dropout_calls": ops._dropout_calls[0], "capture_dropout_calls": self._capture_calls,
+                           "unused_parameters": list(self.unused_parameters) if self.probed else None}}
+
+    def _flat_state(self):
+        flat = getattr(self, "flat_grads", None)
+        return flat if isinstance(flat, FlatState) else None
+
+    def load_state_dict(self, state):
+        """Continue from `state` (state_dict() of this configuration).  Eager, or graph mode after the capture: applied now,
+        in place into the memory the graph reads (flat parameters, moments, bf16 shadows, step_t, lr_factor, the dropout
+        counter) with everything derived from the parameters at capture recomputed in place (PointNet++ packed weights,
+        register_shadows shadows).  Graph mode before the first step: applied right after the set-up steps and the capture,
+        before the first replay, so the set-up steps leave no trace; the capture takes the checkpoint's in-kernel dropout
+        seeds, so the run continues exactly as the saved one would have."""
+        if self.graph_mode and self.graph is None:
+            self._pending_state = state
+            return
+        self._apply_state(state)
+
+    def _seed_capture(self):
+        """The in-kernel dropout seeds are host constants of the captured graph (ops._next_dropout_seed: torch's initial
+        seed and a call counter): capture with those of the checkpoint being resumed, and remember them for the next one."""
+        st = self._pending_state
+        if st is not None and st["native"].get("capture_dropout_calls") is not None:
+            torch.set_rng_state(st["random_states"]["torch_manual_seed"])     # torch.initial_seed() of the saved run
+            ops._dropout_calls[0] = st["native"]["capture_dropout_calls"]
+        self._capture_calls = ops._dropout_calls[0]
+
+    @torch.no_grad()
+    def _apply_state(self, state):
+        from . import checkpoint as C
+        nat = state["native"]
+        if not self.probed and nat.get("unused_parameters") is not None:
+            self._freeze_unused(nat["unused_parameters"])
+        elif self.probed and nat.get("unused_parameters") is not None and \
+                sorted(nat["unused_parameters"]) != sorted(self.unused_parameters):
+            raise ValueError("the checkpoint's unused parameters differ from this step's: another configuration")
+        self.module.model.load_state_dict(state["model"])        # copy_ into the existing (flat-buffer) storage
+        self.module.loss.load_state_dict(state["loss"])
+        moments = C.import_adamw(state["optimizer"], self.module.opt_order, self.optimizer.param_groups)
+        self.total_steps = int(nat["total_steps"])
+        pos = int(state["scheduler"]["last_epoch"])
+        flat = self._flat_state()
+        if flat is not None:
+            steps = {m[0] for m in moments.values() if m is not None}
+            if len(steps) > 1:
+                raise ValueError(f"per-parameter AdamW steps {sorted(steps)}: the flat optimizer keeps one step for all")
+            for p, m in moments.items():
+                o, n = flat.offsets[id(p)], p.numel()
+                flat.exp_avg[o:o + n].copy_(m[1].reshape(-1) if m is not None else torch.zeros(n))
+                flat.exp_avg_sq[o:o + n].copy_(m[2].reshape(-1) if m is not None else torch.zeros(n))
+            flat.step_t.fill_(int(steps.pop()) if steps else 0)
+            flat.shadow.copy_(flat.flat_p)
+        else:
+            C.put_adamw_state(self.optimizer, moments)
+        C.refresh_derived(self.module)
+        if flat is not None:
+            self._check_in_place(flat)
+        if self.scheduler is not None:
+            self.scheduler.load_state_dict(state["scheduler"])
+            for g, lr in zip(self.optimizer.param_groups, self.scheduler.get_last_lr()):
+                g['lr'] = lr
+        else:
+            self._sched_step = pos
+            f = self._lr_lambda(pos)
+            if flat is not None:
+                self.flat_grads.lr_factor.fill_(f)
+            else:
+                for g, base in zip(self.optimizer.param_groups, self._base_lrs):
+                    g['lr'].fill_(base * f)
+        counter = getattr(self, "_step_counter", None)
+        if counter is not None:
+            counter.fill_(nat["dropout_counter"] or 0)
+        C.set_rng_state(state["random_states"])
+        ops._dropout_calls[0] = int(nat["dropout_calls"])
+        self.global_step = int(nat["global_step"])
+        if self.train_log is not None:          # entries of this object's earlier steps are not steps of the resumed run
+            self.train_log.ring.zero_()
+            self.train_log.seen = int(self.train_log.step_counter.item())
+            self.train_log.pending = []
+
+    def _check_in_place(self, flat):
+        """A captured graph reads the flat buffers and the shadows registered at capture: refuse to continue if a parameter
+        no longer lives there (its new values would never reach the graph)."""
+        from .modules.pointnet import PointNetPP
+        base = flat.flat_p.data_ptr()
+        for p in flat.params:
+            if p.data_ptr() != base + 4 * flat.offsets[id(p)]:
+                raise RuntimeError("a parameter was moved out of the flat buffer: the captured graph would train stale weights")
+        for s, p in ops._SHADOW.values():
+            if s.shape != p.shape:
+                raise RuntimeError("a bf16 shadow no longer matches its parameter")
+        for m in self.module.modules():
+            if isinstance(m, PointNetPP) and m._packed is not None and \
+                    m._packed_key != tuple((t.data_ptr(), t._version) for t in list(m.parameters()) + list(m.buffers())):
+                raise RuntimeError("the PointNet++ packed weights were not refreshed")
+
+    def save_state(self, path):
+        """accelerate.save_state layout (sceneverse_b200/checkpoint.py): rank 0 writes the shared files, every rank its
+        random states, then a barrier."""
+        from . import checkpoint as C
+        C.save_state(self, path)
+
+    def load_state(self, path):
+        """Every rank reads the directory written by save_state (its own random states) and load_state_dict()s it."""
+        from . import checkpoint as C
+        self.load_state_dict(C.read_state(path))
+
+    @torch.no_grad()
+    def load_pretrain(self, path):
+        """BaseTrainer.load_pretrain (trainer/build.py:174-184): every pytorch_model*.bin of `path` into the model,
+        strict=False, before the first step.  Returns (missing_keys, unexpected_keys)."""
+        if self.probed:
+            raise RuntimeError("load_pretrain must run before the first step")
+        from . import checkpoint as C
+        return self.module.model.load_state_dict(C.read_pretrain(path), strict=False)
+
     def _lrs(self):
         if self.scheduler is not None:
             return self.scheduler.get_last_lr()
@@ -204,10 +360,15 @@ class PretrainStep:
             self.module.train_log = log
         total.backward()
         unused = [n for n, p in self.module.named_parameters() if p.requires_grad and p.grad is None]
-        for n, p in self.module.named_parameters():
-            if p.requires_grad and p.grad is None:
-                p.requires_grad = False
         self.optimizer.zero_grad(set_to_none=True)
+        self._freeze_unused(unused)
+
+    def _freeze_unused(self, unused):
+        """Freeze the parameters named in `unused` (found by _probe_unused, or read from a checkpoint) and wrap in DDP."""
+        names = set(unused)
+        for n, p in self.module.named_parameters():
+            if n in names:
+                p.requires_grad = False
         for g in self.optimizer.param_groups:
             g['params'] = [p for p in g['params'] if p.requires_grad]
         self.unused_parameters = unused
@@ -342,6 +503,7 @@ class PretrainStep:
                 self._advance_lr()
         cur.wait_stream(side)
         torch.cuda.synchronize(self.device)
+        self._seed_capture()
         from . import _lib
         n0 = _lib.launch_count()
         self.graph = torch.cuda.CUDAGraph()
@@ -366,6 +528,7 @@ class PretrainStep:
                         self._advance_lr()
                     cur.wait_stream(side)
                     torch.cuda.synchronize(self.device)
+                    self._seed_capture()
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g, pool=self.graph.pool()):
                         loss = self._raw_step()       # forward + backward + both all-reduces + clip/AdamW: ONE graph
@@ -388,9 +551,16 @@ class PretrainStep:
         from . import fused_gather
         return all(v is not None for v in fused_gather._state.values())
 
+    def _probe_or_restore(self, data_dict):
+        unused = self._pending_state["native"].get("unused_parameters") if self._pending_state is not None else None
+        if unused is not None:
+            self._freeze_unused(unused)       # the checkpoint's flat layout; no probing pass on the resumed run's batch
+        else:
+            self._probe_unused(data_dict)
+
     def _graph_step(self, data_dict):
         if not self.probed:
-            self._probe_unused(data_dict)
+            self._probe_or_restore(data_dict)
             if self.dp_graph and not self._dp_graph_possible():
                 self.graph_mode = self.dp_graph = False
                 self.use_ddp = True
@@ -399,9 +569,15 @@ class PretrainStep:
                     gradient_as_bucket_view=True, bucket_cap_mb=64)
                 if self.train_log is not None:
                     self.train_log.step_counter, self.train_log.advance = self.train_log.own_step, True
+                if self._pending_state is not None:
+                    st, self._pending_state = self._pending_state, None
+                    self._apply_state(st)
                 return self._step(data_dict)
         if self.graph is None:
             self._capture(data_dict)
+            if self._pending_state is not None:     # undo the set-up steps: the first replay continues the checkpoint
+                st, self._pending_state = self._pending_state, None
+                self._apply_state(st)
         for k, dst in self.static_batch.items():
             src = data_dict[k]
             if src.data_ptr() != dst.data_ptr():
@@ -459,7 +635,7 @@ class PretrainStep:
         if self.graph_mode:
             return self._graph_step(data_dict)
         if not self.probed:
-            self._probe_unused(data_dict)
+            self._probe_or_restore(data_dict)
         net = self.ddp if self.ddp is not None else self.module
         self.optimizer.zero_grad(set_to_none=True)
         with torch.autocast(self.device.type, dtype=self.dtype, enabled=self.dtype != torch.float32):
@@ -652,6 +828,56 @@ class ObjClsStep:
         self.optimizer = torch.optim.AdamW(self.model.parameters(), lr=torch.tensor(lr, device=self.device) if self.graph_mode else lr,
                                            fused=self.device.type == "cuda", capturable=self.graph_mode)
         self.graph = self.static_batch = self.static_loss = None
+        self.lr = lr
+        self.global_step = 0
+        self._pending_state = None
+
+    # ---- checkpoints: the layout and forms of PretrainStep's (sceneverse_b200/checkpoint.py) ------------------------------
+    def state_dict(self):
+        """`model` (PointNet++ with the BatchNorm running statistics, the text embeddings), `loss` (empty: the label-smoothed
+        CE has no parameters), `optimizer` (torch AdamW form, one group over model.parameters()), `scheduler` (constant lr,
+        LambdaLR form), `random_states`, `native` (global_step)."""
+        if self._pending_state is not None:
+            return self._pending_state
+        from . import checkpoint as C
+
+        def moments(p):
+            st = self.optimizer.state.get(p)
+            if not st:
+                return None
+            return float(st["step"]), C.to_cpu(st["exp_avg"]), C.to_cpu(st["exp_avg_sq"])
+        order = [list(self.model.parameters())]
+        return {"model": C.to_cpu(self.model.state_dict()), "loss": {},
+                "optimizer": C.export_adamw(order, self.optimizer.param_groups, [self.lr], [self.lr], moments),
+                "scheduler": C.lambda_lr_state([self.lr], self.global_step, [self.lr]), "random_states": C.rng_state(),
+                "native": {"global_step": self.global_step, "total_steps": None, "dropout_counter": None,
+                           "dropout_calls": None, "capture_dropout_calls": None, "unused_parameters": []}}
+
+    def load_state_dict(self, state):
+        """As PretrainStep.load_state_dict: in place now, or (graph mode, before the first step) after the set-up steps and
+        the capture, before the first replay."""
+        if self.graph_mode and self.graph is None:
+            self._pending_state = state
+            return
+        self._apply_state(state)
+
+    @torch.no_grad()
+    def _apply_state(self, state):
+        from . import checkpoint as C
+        self.model.load_state_dict(state["model"])
+        order = [list(self.model.parameters())]
+        C.put_adamw_state(self.optimizer, C.import_adamw(state["optimizer"], order, self.optimizer.param_groups))
+        C.refresh_derived(self.model)
+        C.set_rng_state(state["random_states"])
+        self.global_step = int(state["native"]["global_step"])
+
+    def save_state(self, path):
+        from . import checkpoint as C
+        C.save_state(self, path)
+
+    def load_state(self, path):
+        from . import checkpoint as C
+        self.load_state_dict(C.read_state(path))
 
     def _fwd_bwd(self, batch):
         if self.flat_grads is not None:
@@ -672,6 +898,7 @@ class ObjClsStep:
         return loss
 
     def step(self, batch):
+        self.global_step += 1
         if not self.graph_mode:
             return self._raw(batch)
         if self.graph is None:
@@ -697,6 +924,10 @@ class ObjClsStep:
                 with torch.cuda.graph(self.graph_opt, pool=self.graph.pool()):
                     self.optimizer.step()
             self.native_launches_per_step = _lib.launch_count() - n0
+            if self._pending_state is not None:     # undo the set-up steps: the first replay continues the checkpoint
+                st, self._pending_state = self._pending_state, None
+                self._apply_state(st)
+                self.global_step += 1
         for k, dst in self.static_batch.items():
             if batch[k].data_ptr() != dst.data_ptr():
                 dst.copy_(batch[k], non_blocking=True)
