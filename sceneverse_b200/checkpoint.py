@@ -94,6 +94,16 @@ def export_adamw(order, live_groups, lrs, base_lrs, moments):
     return {"state": state, "param_groups": groups}
 
 
+def adamw_moments(optimizer):
+    """export_adamw's moments(p) for a torch AdamW: its own per-parameter state, copied to the host."""
+    def moments(p):
+        st = optimizer.state.get(p)
+        if not st:
+            return None
+        return float(st["step"]), to_cpu(st["exp_avg"]), to_cpu(st["exp_avg_sq"])
+    return moments
+
+
 def import_adamw(sd, order, live_groups):
     """Inverse of export_adamw: {parameter: (step, exp_avg, exp_avg_sq) or None} for every parameter of `live_groups`."""
     flat = [p for g in order for p in g]
@@ -138,8 +148,8 @@ def put_adamw_state(optimizer, moments):
 
 
 def lambda_lr_state(base_lrs, position, last_lrs):
-    """torch LambdaLR.state_dict() of a schedule at `position` (for the graph-mode steps, whose schedule lives in
-    PretrainStep._sched_step and a device lr factor instead of a LambdaLR)."""
+    """torch LambdaLR.state_dict() of a schedule at `position` (the training steps keep the position as an integer instead
+    of a LambdaLR)."""
     return {"base_lrs": [float(b) for b in base_lrs], "last_epoch": int(position), "_step_count": int(position) + 1,
             "_is_initial": False, "_get_lr_called_within_step": False, "_last_lr": [float(x) for x in last_lrs],
             "lr_lambdas": [None] * len(base_lrs)}

@@ -112,7 +112,87 @@ class TrainLog:
         return out
 
 
-class PretrainStep:
+class CapturedStep:
+    """The CUDA-graph path PretrainStep and ObjClsStep share: static input buffers, eager set-up steps on a side stream, the
+    capture (one graph, or with several ranks graph A | NCCL mean of flat_grads | graph B), the replay, and a checkpoint
+    loaded before the capture applied right after it.  Subclasses set `device` and `graph_mode` and define `_apply_state`."""
+    graph = graph_opt = static_batch = static_loss = flat_grads = None
+    _pending_state = None             # a checkpoint loaded before the first graph-mode step
+
+    def load_state_dict(self, state):
+        """Continue from `state` (state_dict() of this configuration).  Eager, or graph mode after the capture: applied now,
+        in place into the memory the graph reads.  Graph mode before the first step: applied right after the set-up steps
+        and the capture, before the first replay, so the set-up steps leave no trace."""
+        if self.graph_mode and self.graph is None:
+            self._pending_state = state
+            return
+        self._apply_state(state)
+
+    def _apply_pending(self):
+        """Apply the checkpoint loaded before the capture, if any (the first replay continues it); True if there was one."""
+        if self._pending_state is None:
+            return False
+        st, self._pending_state = self._pending_state, None
+        self._apply_state(st)
+        return True
+
+    def save_state(self, path):
+        """accelerate.save_state layout (sceneverse_b200/checkpoint.py): rank 0 writes the shared files, every rank its
+        random states, then a barrier."""
+        from . import checkpoint as C
+        C.save_state(self, path)
+
+    def load_state(self, path):
+        """Every rank reads the directory written by save_state (its own random states) and load_state_dict()s it."""
+        from . import checkpoint as C
+        self.load_state_dict(C.read_state(path))
+
+    def _copy_in(self, batch):
+        """Put `batch` into the static input buffers the graphs read (the first call makes them); an input that already is
+        the static buffer is not copied."""
+        if self.static_batch is None:
+            self.static_batch = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
+            return
+        for k, dst in self.static_batch.items():
+            if batch[k].data_ptr() != dst.data_ptr():
+                dst.copy_(batch[k], non_blocking=True)
+
+    def _side_steps(self, step, n):
+        """n calls of step() on a side stream, then a device synchronise: real optimisation steps before a capture, which
+        allocate gradient and optimizer state outside the graph pool."""
+        cur = torch.cuda.current_stream(self.device)
+        side = torch.cuda.Stream(self.device)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            for _ in range(n):
+                step()
+        cur.wait_stream(side)
+        torch.cuda.synchronize(self.device)
+
+    def _capture_graphs(self, step, opt=None):
+        """Capture step() (it returns the loss) as `graph`; with `opt`, step() is forward + backward only and opt() is
+        captured as `graph_opt` in the same pool, and _replay all-reduces flat_grads between the two.  Counts the native
+        kernel launches one replay makes."""
+        from . import _lib
+        n0 = _lib.launch_count()
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self.static_loss = step()
+        if opt is not None:
+            self.graph_opt = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph_opt, pool=self.graph.pool()):
+                opt()
+        self.native_launches_per_step = _lib.launch_count() - n0
+
+    def _replay(self):
+        self.graph.replay()
+        if self.graph_opt is not None:
+            self.flat_grads.all_reduce_mean()
+            self.graph_opt.replay()
+        return self.static_loss
+
+
+class PretrainStep(CapturedStep):
     def __init__(self, cfg, device, total_steps=100000, dtype=torch.bfloat16, ddp=None, seed=0, cuda_graph=False,
                  overlap_allreduce=False, train_eval=None, log_every=100):
         """cuda_graph=True (single process, CUDA): after a few eager steps the whole step — forward, losses, backward,
@@ -155,23 +235,19 @@ class PretrainStep:
         mr = self.cfg.solver.sched.args.get("minimum_ratio", 1e-5)
         self.total_steps = total_steps         # read at every evaluation: a loaded checkpoint restores it
         self._lr_lambda = lambda s: M.warmup_cosine(s, warm, self.total_steps, minimum_ratio=mr)
-        self._pending_state = None             # a checkpoint loaded before the first graph-mode step
         self._capture_calls = None             # ops._dropout_calls when the replayed graph was captured
+        # the warm-up/cosine schedule is its position _sched_step and the base lrs (_set_lrs); in graph mode the torch AdamW
+        # holds the parameter groups but never steps: FlatState.optimizer_step does
+        self.optimizer = torch.optim.AdamW(groups, lr=self.cfg.solver.lr, fused=self.device.type == "cuda", **kw)
+        for g in self.optimizer.param_groups:       # each group's base lr, where torch's lr schedulers keep it
+            g['initial_lr'] = g['lr']
+        self._base_lrs = [float(g['initial_lr']) for g in self.optimizer.param_groups]
+        self._sched_step = 0
+        self._set_lrs()
         if self.graph_mode:
-            # capturable AdamW reads lr from a device tensor; the warm-up/cosine schedule fills it from the host per step
-            self._base_lrs = [float(g.get('lr', self.cfg.solver.lr)) for g in groups]
-            for g in groups:
-                g['lr'] = torch.tensor(float(g.get('lr', self.cfg.solver.lr)) * self._lr_lambda(0), device=self.device)
-            self.optimizer = torch.optim.AdamW(groups, fused=True, capturable=True, **kw)
-            self.scheduler = None
-            self._sched_step = 0
             self._step_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
             from . import _lib
             _lib.check(_lib.gps(), _lib.gps().sv_dropout_seed_offset(self._step_counter.data_ptr()), "sv_dropout_seed_offset")
-            self.graph = self.graph_opt = self.static_batch = self.static_loss = self.flat_grads = None
-        else:
-            self.optimizer = torch.optim.AdamW(groups, lr=self.cfg.solver.lr, fused=self.device.type == "cuda", **kw)
-            self.scheduler = torch.optim.lr_scheduler.LambdaLR(self.optimizer, self._lr_lambda)
         self.grad_norm = self.cfg.solver.get("grad_norm")
         self.ddp = None
         self.probed = False
@@ -196,12 +272,12 @@ class PretrainStep:
     def state_dict(self):
         """Everything a resumed run needs, on the host, independent of the flat layout: `model` / `loss` (state_dicts with
         the reference's keys), `optimizer` (torch AdamW.state_dict() form, parameter indices in get_opt_params() order, loss
-        group last), `scheduler` (LambdaLR form), `random_states` (this rank's generators) and `native` (global_step,
+        group last), `scheduler` (checkpoint.lambda_lr_state), `random_states` (this rank's generators) and `native` (global_step,
         total_steps, the device dropout counter, the in-kernel dropout seed position, the probed unused parameters)."""
         if self._pending_state is not None:          # loaded, not applied yet: that state is this step's state
             return self._pending_state
         from . import checkpoint as C
-        flat = self._flat_state()
+        flat = self.flat_grads
         if flat is not None:
             step = int(flat.step_t.item())
             host = {name: getattr(flat, name).cpu() for name in ("exp_avg", "exp_avg_sq")}
@@ -210,15 +286,9 @@ class PretrainStep:
                 o, n = flat.offsets[id(p)], p.numel()
                 return step, host["exp_avg"][o:o + n].view(p.shape).clone(), host["exp_avg_sq"][o:o + n].view(p.shape).clone()
         else:
-            def moments(p):
-                st = self.optimizer.state.get(p)
-                if not st:
-                    return None
-                return float(st["step"]), C.to_cpu(st["exp_avg"]), C.to_cpu(st["exp_avg_sq"])
-        base = self._base_lrs if self.scheduler is None else self.scheduler.base_lrs
-        optim = C.export_adamw(self.module.opt_order, self.optimizer.param_groups, self._lrs(), base, moments)
-        sched = self.scheduler.state_dict() if self.scheduler is not None else \
-            C.lambda_lr_state(self._base_lrs, self._sched_step, self._lrs())
+            moments = C.adamw_moments(self.optimizer)
+        optim = C.export_adamw(self.module.opt_order, self.optimizer.param_groups, self._lrs(), self._base_lrs, moments)
+        sched = C.lambda_lr_state(self._base_lrs, self._sched_step, self._lrs())
         counter = getattr(self, "_step_counter", None)
         return {"model": C.to_cpu(self.module.model.state_dict()), "loss": C.to_cpu(self.module.loss.state_dict()),
                 "optimizer": optim, "scheduler": sched, "random_states": C.rng_state(),
@@ -226,22 +296,6 @@ class PretrainStep:
                            "dropout_counter": int(counter.item()) if counter is not None else None,
                            "dropout_calls": ops._dropout_calls[0], "capture_dropout_calls": self._capture_calls,
                            "unused_parameters": list(self.unused_parameters) if self.probed else None}}
-
-    def _flat_state(self):
-        flat = getattr(self, "flat_grads", None)
-        return flat if isinstance(flat, FlatState) else None
-
-    def load_state_dict(self, state):
-        """Continue from `state` (state_dict() of this configuration).  Eager, or graph mode after the capture: applied now,
-        in place into the memory the graph reads (flat parameters, moments, bf16 shadows, step_t, lr_factor, the dropout
-        counter) with everything derived from the parameters at capture recomputed in place (PointNet++ packed weights,
-        register_shadows shadows).  Graph mode before the first step: applied right after the set-up steps and the capture,
-        before the first replay, so the set-up steps leave no trace; the capture takes the checkpoint's in-kernel dropout
-        seeds, so the run continues exactly as the saved one would have."""
-        if self.graph_mode and self.graph is None:
-            self._pending_state = state
-            return
-        self._apply_state(state)
 
     def _seed_capture(self):
         """The in-kernel dropout seeds are host constants of the captured graph (ops._next_dropout_seed: torch's initial
@@ -254,6 +308,11 @@ class PretrainStep:
 
     @torch.no_grad()
     def _apply_state(self, state):
+        """load_state_dict's work.  After the capture it writes in place into what the graph reads (flat parameters,
+        moments, bf16 shadows, step_t, lr_factor, the dropout counter) and recomputes in place everything derived from the
+        parameters at capture (PointNet++ packed weights, register_shadows shadows).  A checkpoint loaded before the first
+        graph-mode step also gave the capture its in-kernel dropout seeds (_seed_capture), so the run continues exactly as
+        the saved one would have."""
         from . import checkpoint as C
         nat = state["native"]
         if not self.probed and nat.get("unused_parameters") is not None:
@@ -265,8 +324,7 @@ class PretrainStep:
         self.module.loss.load_state_dict(state["loss"])
         moments = C.import_adamw(state["optimizer"], self.module.opt_order, self.optimizer.param_groups)
         self.total_steps = int(nat["total_steps"])
-        pos = int(state["scheduler"]["last_epoch"])
-        flat = self._flat_state()
+        flat = self.flat_grads
         if flat is not None:
             steps = {m[0] for m in moments.values() if m is not None}
             if len(steps) > 1:
@@ -282,18 +340,8 @@ class PretrainStep:
         C.refresh_derived(self.module)
         if flat is not None:
             self._check_in_place(flat)
-        if self.scheduler is not None:
-            self.scheduler.load_state_dict(state["scheduler"])
-            for g, lr in zip(self.optimizer.param_groups, self.scheduler.get_last_lr()):
-                g['lr'] = lr
-        else:
-            self._sched_step = pos
-            f = self._lr_lambda(pos)
-            if flat is not None:
-                self.flat_grads.lr_factor.fill_(f)
-            else:
-                for g, base in zip(self.optimizer.param_groups, self._base_lrs):
-                    g['lr'].fill_(base * f)
+        self._sched_step = int(state["scheduler"]["last_epoch"])
+        self._set_lrs()
         counter = getattr(self, "_step_counter", None)
         if counter is not None:
             counter.fill_(nat["dropout_counter"] or 0)
@@ -321,17 +369,6 @@ class PretrainStep:
                     m._packed_key != tuple((t.data_ptr(), t._version) for t in list(m.parameters()) + list(m.buffers())):
                 raise RuntimeError("the PointNet++ packed weights were not refreshed")
 
-    def save_state(self, path):
-        """accelerate.save_state layout (sceneverse_b200/checkpoint.py): rank 0 writes the shared files, every rank its
-        random states, then a barrier."""
-        from . import checkpoint as C
-        C.save_state(self, path)
-
-    def load_state(self, path):
-        """Every rank reads the directory written by save_state (its own random states) and load_state_dict()s it."""
-        from . import checkpoint as C
-        self.load_state_dict(C.read_state(path))
-
     @torch.no_grad()
     def load_pretrain(self, path):
         """BaseTrainer.load_pretrain (trainer/build.py:174-184): every pytorch_model*.bin of `path` into the model,
@@ -342,10 +379,20 @@ class PretrainStep:
         return self.module.model.load_state_dict(C.read_pretrain(path), strict=False)
 
     def _lrs(self):
-        if self.scheduler is not None:
-            return self.scheduler.get_last_lr()
+        return [g['lr'] for g in self.optimizer.param_groups]
+
+    def _set_lrs(self):
+        """The schedule at _sched_step: base lr * factor into the param groups (the lrs the eager AdamW reads and the logs
+        and checkpoints report) and, once the flat state exists, the factor into FlatState.lr_factor (the captured AdamW's)."""
         f = self._lr_lambda(self._sched_step)
-        return [base * f for base in self._base_lrs]
+        for g, base in zip(self.optimizer.param_groups, self._base_lrs):
+            g['lr'] = base * f
+        if self.flat_grads is not None:
+            self.flat_grads.lr_factor.fill_(f)
+
+    def _advance_lr(self):
+        self._sched_step += 1
+        self._set_lrs()
 
     def _probe_unused(self, data_dict):
         """One local forward/backward to find the parameters this configuration never touches (e.g. the object LM head
@@ -373,10 +420,13 @@ class PretrainStep:
             g['params'] = [p for p in g['params'] if p.requires_grad]
         self.unused_parameters = unused
         if self.use_ddp:
-            self.ddp = nn.parallel.DistributedDataParallel(
-                self.module, device_ids=[self.device.index] if self.device.type == "cuda" else None,
-                find_unused_parameters=False, gradient_as_bucket_view=True, bucket_cap_mb=64)
+            self._wrap_ddp()
         self.probed = True
+
+    def _wrap_ddp(self):
+        self.ddp = nn.parallel.DistributedDataParallel(
+            self.module, device_ids=[self.device.index] if self.device.type == "cuda" else None,
+            find_unused_parameters=False, gradient_as_bucket_view=True, bucket_cap_mb=64)
 
     def parameters(self):
         return [p for p in self.module.parameters() if p.requires_grad]
@@ -402,14 +452,9 @@ class PretrainStep:
     # ---- CUDA-graph path ---------------------------------------------------------------------------------------------
     def _raw_fwd_bwd(self):
         self._step_counter.add_(1)
-        if self.flat_grads is not None:
-            self.flat_grads.zero()
-        else:
-            self.optimizer.zero_grad(set_to_none=False)
-        if self.flat_grads is None or not isinstance(self.flat_grads, FlatState):
-            ops.refresh_shadows()
+        self.flat_grads.zero()
         # gradients live in the flat buffer: the wgrad kernels accumulate into it directly (no AccumulateGrad adds)
-        prev, ops.DIRECT_GRAD[0] = ops.DIRECT_GRAD[0], self.flat_grads is not None
+        prev, ops.DIRECT_GRAD[0] = ops.DIRECT_GRAD[0], True
         self._ar_work = None
         self.module.model._lang_grad_hook = self._early_allreduce if self._overlap_now else None
         try:
@@ -441,25 +486,14 @@ class PretrainStep:
             self.flat_grads.all_reduce_mean()
         self._ar_work = None
 
-    def _raw_opt(self):
-        if isinstance(self.flat_grads, FlatState):
-            self.flat_grads.optimizer_step()                    # native: clip + AdamW + bf16 shadows, one pass
-            return
-        if self.grad_norm is not None:
-            if self.flat_grads is not None:
-                self.flat_grads.clip_norm_(self.grad_norm)     # same math as clip_grad_norm_, two kernels on the flat buffer
-            else:
-                torch.nn.utils.clip_grad_norm_(self.parameters(), self.grad_norm, foreach=True)
-        self.optimizer.step()
-
     def _raw_step(self):
+        """One step of what the graph records, run eagerly on the flat state."""
         loss = self._raw_fwd_bwd()
-        if self.flat_grads is not None:
-            if self._overlap_now:
-                self._finish_allreduce()
-            else:
-                self.flat_grads.all_reduce_mean()
-        self._raw_opt()
+        if self._overlap_now:
+            self._finish_allreduce()
+        else:
+            self.flat_grads.all_reduce_mean()
+        self.flat_grads.optimizer_step()                    # native: clip + AdamW + bf16 shadows, one pass
         return loss
 
     def _lang_boundary(self):
@@ -473,61 +507,39 @@ class PretrainStep:
             return None
         return (end_lang + 7) // 8 * 8 if (end_lang + 7) // 8 * 8 <= first_other else end_lang
 
-    def _advance_lr(self):
-        self._sched_step += 1
-        f = self._lr_lambda(self._sched_step)
-        if isinstance(self.flat_grads, FlatState):
-            self.flat_grads.lr_factor.fill_(f)
-            return
-        for g, base in zip(self.optimizer.param_groups, self._base_lrs):
-            g['lr'].fill_(base * f)
-
-    def _capture(self, data_dict):
-        self.static_batch = {k: v.clone() for k, v in data_dict.items() if torch.is_tensor(v)}
-        if self.dp_graph:
-            sync_module_state(self.module)
-        ops.clear_shadows()
+    def _make_flat_state(self):
+        """The graph path's optimizer: the trainable parameters, their gradients, AdamW moments and bf16 shadows moved
+        into one FlatState (flat_grads) at the schedule's current lr, and the packed sibling projections registered."""
         kw = dict(self.cfg.solver.optim.args)
         self.flat_grads = FlatState(self.optimizer.param_groups, self._base_lrs, betas=tuple(kw.get("betas", (0.9, 0.999))),
                                     eps=float(kw.get("eps", 1e-8)), max_norm=self.grad_norm)
-        self.flat_grads.lr_factor.fill_(self._lr_lambda(self._sched_step))
+        self._set_lrs()
         register_packs(self.module, self.flat_grads)
+
+    def _set_up_step(self):
+        self._raw_step()
+        self._advance_lr()
+
+    def _capture(self, data_dict):
+        self._copy_in(data_dict)
+        if self.dp_graph:
+            sync_module_state(self.module)
+        ops.clear_shadows()
+        self._make_flat_state()
         if self.dtype == torch.bfloat16:
             ops.register_shadows(self.module)       # whatever bf16 linears read outside the flat buffer (frozen parameters)
-        cur = torch.cuda.current_stream(self.device)
-        side = torch.cuda.Stream(self.device)
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            for _ in range(3):          # real optimisation steps: allocates grads / optimizer state outside the graph pool
-                self._raw_step()
-                self._advance_lr()
-        cur.wait_stream(side)
-        torch.cuda.synchronize(self.device)
+        self._side_steps(self._set_up_step, 3)
         self._seed_capture()
-        from . import _lib
-        n0 = _lib.launch_count()
-        self.graph = torch.cuda.CUDAGraph()
-        if not self.dp_graph:
-            with torch.cuda.graph(self.graph):
-                self.static_loss = self._raw_step()
+        if self.dp_graph:
+            self._capture_graphs(self._raw_fwd_bwd, self.flat_grads.optimizer_step)
         else:
-            with torch.cuda.graph(self.graph):
-                self.static_loss = self._raw_fwd_bwd()
-            self.graph_opt = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph_opt, pool=self.graph.pool()):
-                self._raw_opt()
-        self.native_launches_per_step = _lib.launch_count() - n0   # native kernel nodes replayed per step
+            self._capture_graphs(self._raw_step)
         if self.dp_graph and self.overlap_allreduce:
             self._lang_end = self._lang_boundary()
             if self._lang_end is not None:
                 try:
                     self._overlap_now = True
-                    side.wait_stream(cur)
-                    with torch.cuda.stream(side):       # one eager step through the hook path (NCCL warm-up on its stream)
-                        self._raw_step()
-                        self._advance_lr()
-                    cur.wait_stream(side)
-                    torch.cuda.synchronize(self.device)
+                    self._side_steps(self._set_up_step, 1)     # one eager step through the hook path (NCCL warm-up)
                     self._seed_capture()
                     g = torch.cuda.CUDAGraph()
                     with torch.cuda.graph(g, pool=self.graph.pool()):
@@ -561,37 +573,25 @@ class PretrainStep:
     def _graph_step(self, data_dict):
         if not self.probed:
             self._probe_or_restore(data_dict)
-            if self.dp_graph and not self._dp_graph_possible():
+            if self.dp_graph and not self._dp_graph_possible():      # the eager data-parallel step from here on
                 self.graph_mode = self.dp_graph = False
                 self.use_ddp = True
-                self.ddp = nn.parallel.DistributedDataParallel(
-                    self.module, device_ids=[self.device.index], find_unused_parameters=False,
-                    gradient_as_bucket_view=True, bucket_cap_mb=64)
+                self._wrap_ddp()
                 if self.train_log is not None:
                     self.train_log.step_counter, self.train_log.advance = self.train_log.own_step, True
-                if self._pending_state is not None:
-                    st, self._pending_state = self._pending_state, None
-                    self._apply_state(st)
+                self._apply_pending()
                 return self._step(data_dict)
         if self.graph is None:
             self._capture(data_dict)
-            if self._pending_state is not None:     # undo the set-up steps: the first replay continues the checkpoint
-                st, self._pending_state = self._pending_state, None
-                self._apply_state(st)
-        for k, dst in self.static_batch.items():
-            src = data_dict[k]
-            if src.data_ptr() != dst.data_ptr():
-                dst.copy_(src, non_blocking=True)
+            self._apply_pending()
+        self._copy_in(data_dict)
         if self.overlapped:
             self.graph_overlap.replay()
             self._advance_lr()
             return self.static_loss_overlap
-        self.graph.replay()
-        if self.dp_graph:
-            self.flat_grads.all_reduce_mean()
-            self.graph_opt.replay()
+        loss = self._replay()
         self._advance_lr()
-        return self.static_loss
+        return loss
 
     def phase_times(self, data_dict, steps=5):
         """(ms_fwd_bwd, ms_allreduce, ms_opt) of the NON-overlapped data-parallel step (graph | NCCL | graph), CUDA events on
@@ -599,9 +599,7 @@ class PretrainStep:
         assert self.dp_graph and self.graph is not None and self.graph_opt is not None
         warm = 3                      # un-timed: the ranks fall into step (the exchange kernel waits for the slowest peer)
         ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(warm + steps)]
-        for k, dst in self.static_batch.items():
-            if data_dict[k].data_ptr() != dst.data_ptr():
-                dst.copy_(data_dict[k], non_blocking=True)
+        self._copy_in(data_dict)
         torch.cuda.synchronize(self.device)
         dist.barrier()
         for e in ev:
@@ -644,10 +642,7 @@ class PretrainStep:
         if self.grad_norm is not None:
             torch.nn.utils.clip_grad_norm_(self.parameters(), self.grad_norm, foreach=True)
         self.optimizer.step()
-        if self.scheduler is not None:
-            self.scheduler.step()
-        else:                       # capturable optimizer (graph mode was requested but is not possible): tensor lr
-            self._advance_lr()
+        self._advance_lr()
         return total.detach()
 
 
@@ -666,13 +661,6 @@ class FlatGrads:
 
     def zero(self):
         self.flat.zero_()
-
-    def clip_norm_(self, max_norm, eps=1e-6):
-        """torch.nn.utils.clip_grad_norm_ (L2) on the flat buffer: the norm of the per-tensor norms is the norm of the
-        concatenation."""
-        total = torch.linalg.vector_norm(self.flat, 2.0)
-        self.flat.mul_((max_norm / (total + eps)).clamp(max=1.0))
-        return total
 
     def all_reduce_mean(self, group=None):
         if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
@@ -797,7 +785,7 @@ def batch_to_device(np_batch, device, pinned=None, non_blocking=True):
     return out
 
 
-class ObjClsStep:
+class ObjClsStep(CapturedStep):
     """Object-level pre-training step (reference: model/objcls.py:64-98 + optim/loss/loss.py:96-102, BASELINE.json configs[1]):
     PointNet++ TRAINABLE with train-mode BatchNorm -> dropout -> 607-way open-vocabulary logits -> label-smoothed CE ->
     AdamW.  The point operators and their gradients (group_points_grad / gather) are the native kernels; conv / BatchNorm
@@ -815,7 +803,7 @@ class ObjClsStep:
         self.device, self.dtype = torch.device(device), dtype
         self.model = M.ObjCls({"num_gpu": num_gpu, "solver": {"lr": lr}}, text_embeds=text_embeds).to(self.device).train()
         self.graph_mode = bool(cuda_graph) and self.device.type == "cuda"
-        self.ddp = self.flat_grads = self.graph_opt = None
+        self.ddp = None
         if num_gpu > 1 and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
             from . import pn_train
             sync_module_state(self.model)
@@ -827,10 +815,8 @@ class ObjClsStep:
                     self.model, device_ids=[self.device.index] if self.device.type == "cuda" else None)
         self.optimizer = torch.optim.AdamW(self.model.parameters(), lr=torch.tensor(lr, device=self.device) if self.graph_mode else lr,
                                            fused=self.device.type == "cuda", capturable=self.graph_mode)
-        self.graph = self.static_batch = self.static_loss = None
         self.lr = lr
         self.global_step = 0
-        self._pending_state = None
 
     # ---- checkpoints: the layout and forms of PretrainStep's (sceneverse_b200/checkpoint.py) ------------------------------
     def state_dict(self):
@@ -840,26 +826,13 @@ class ObjClsStep:
         if self._pending_state is not None:
             return self._pending_state
         from . import checkpoint as C
-
-        def moments(p):
-            st = self.optimizer.state.get(p)
-            if not st:
-                return None
-            return float(st["step"]), C.to_cpu(st["exp_avg"]), C.to_cpu(st["exp_avg_sq"])
         order = [list(self.model.parameters())]
         return {"model": C.to_cpu(self.model.state_dict()), "loss": {},
-                "optimizer": C.export_adamw(order, self.optimizer.param_groups, [self.lr], [self.lr], moments),
+                "optimizer": C.export_adamw(order, self.optimizer.param_groups, [self.lr], [self.lr],
+                                            C.adamw_moments(self.optimizer)),
                 "scheduler": C.lambda_lr_state([self.lr], self.global_step, [self.lr]), "random_states": C.rng_state(),
                 "native": {"global_step": self.global_step, "total_steps": None, "dropout_counter": None,
                            "dropout_calls": None, "capture_dropout_calls": None, "unused_parameters": []}}
-
-    def load_state_dict(self, state):
-        """As PretrainStep.load_state_dict: in place now, or (graph mode, before the first step) after the set-up steps and
-        the capture, before the first replay."""
-        if self.graph_mode and self.graph is None:
-            self._pending_state = state
-            return
-        self._apply_state(state)
 
     @torch.no_grad()
     def _apply_state(self, state):
@@ -870,14 +843,6 @@ class ObjClsStep:
         C.refresh_derived(self.model)
         C.set_rng_state(state["random_states"])
         self.global_step = int(state["native"]["global_step"])
-
-    def save_state(self, path):
-        from . import checkpoint as C
-        C.save_state(self, path)
-
-    def load_state(self, path):
-        from . import checkpoint as C
-        self.load_state_dict(C.read_state(path))
 
     def _fwd_bwd(self, batch):
         if self.flat_grads is not None:
@@ -902,37 +867,14 @@ class ObjClsStep:
         if not self.graph_mode:
             return self._raw(batch)
         if self.graph is None:
-            self.static_batch = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
-            cur = torch.cuda.current_stream(self.device)
-            side = torch.cuda.Stream(self.device)
-            side.wait_stream(cur)
-            with torch.cuda.stream(side):
-                for _ in range(3):
-                    self._raw(self.static_batch)
-            cur.wait_stream(side)
-            torch.cuda.synchronize(self.device)
-            from . import _lib
-            n0 = _lib.launch_count()
-            self.graph = torch.cuda.CUDAGraph()
+            self._copy_in(batch)
+            static = self.static_batch
+            self._side_steps(lambda: self._raw(static), 3)
             if self.flat_grads is None:
-                with torch.cuda.graph(self.graph):
-                    self.static_loss = self._raw(self.static_batch)
+                self._capture_graphs(lambda: self._raw(static))
             else:
-                with torch.cuda.graph(self.graph):
-                    self.static_loss = self._fwd_bwd(self.static_batch)
-                self.graph_opt = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(self.graph_opt, pool=self.graph.pool()):
-                    self.optimizer.step()
-            self.native_launches_per_step = _lib.launch_count() - n0
-            if self._pending_state is not None:     # undo the set-up steps: the first replay continues the checkpoint
-                st, self._pending_state = self._pending_state, None
-                self._apply_state(st)
+                self._capture_graphs(lambda: self._fwd_bwd(static), self.optimizer.step)
+            if self._apply_pending():       # the checkpoint's global_step counts the steps before this one
                 self.global_step += 1
-        for k, dst in self.static_batch.items():
-            if batch[k].data_ptr() != dst.data_ptr():
-                dst.copy_(batch[k], non_blocking=True)
-        self.graph.replay()
-        if self.graph_opt is not None:
-            self.flat_grads.all_reduce_mean()
-            self.graph_opt.replay()
-        return self.static_loss
+        self._copy_in(batch)
+        return self._replay()

@@ -17,14 +17,14 @@ TF = weights.synthetic_tensor("text_features", (607, 768))
 
 
 def cpu_step(seed, opt_step=True):
-    """A CPU fp32 GPS step; opt_step: one AdamW / scheduler step on seeded random gradients, so the optimizer has state."""
+    """A CPU fp32 GPS step; opt_step: one AdamW / schedule step on seeded random gradients, so the optimizer has state."""
     ps = train.PretrainStep(M.pretrain_config(1, text_features=TF), "cpu", dtype=torch.float32, seed=seed)
     if opt_step:
         g = torch.Generator().manual_seed(seed + 1)
         for p in ps.parameters():
             p.grad = torch.randn(p.shape, generator=g) * 1e-2
         ps.optimizer.step()
-        ps.scheduler.step()
+        ps._advance_lr()
         ps.global_step += 1
     return ps
 
@@ -56,6 +56,22 @@ def test_layout_and_eager_round_trip(tmp_path):
     assert set(checkpoint.read_pretrain(tmp_path)) == set(want["model"]) | set(want["loss"])
     with pytest.raises(FileNotFoundError):
         checkpoint.read_pretrain(tmp_path / "missing")
+    # the schedule is torch's LambdaLR over the same groups and lambda: the same lrs and the same saved `scheduler` dict,
+    # through the warm-up and the cosine
+    cfg = M.pretrain_config(1, text_features=TF)
+    cfg["solver"]["sched"]["args"]["warmup_steps"] = 3
+    r = train.PretrainStep(cfg, "cpu", total_steps=10, dtype=torch.float32, seed=2)
+    groups = r.module.model.get_opt_params() + [{"params": list(r.module.loss.parameters()), "weight_decay": 0.0}]
+    opt = torch.optim.AdamW(groups, lr=r.cfg.solver.lr)
+    lam = torch.optim.lr_scheduler.LambdaLR(opt, r._lr_lambda)
+    for i in range(11):
+        assert [g["lr"] for g in r.optimizer.param_groups] == lam.get_last_lr(), i
+        if i in (0, 10):
+            assert r.state_dict()["scheduler"] == lam.state_dict(), i
+        r.optimizer.step()
+        r._advance_lr()
+        opt.step()
+        lam.step()
 
 
 def test_objcls_to_gps_vision_path(tmp_path):

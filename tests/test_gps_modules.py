@@ -281,11 +281,7 @@ def test_graph_step_matches_eager_step_parameters():
     # graph path: the same single step, run eagerly on the flat state (what the capture records)
     graph.static_batch = {k: v.clone() for k, v in batch.items()}
     from sceneverse_b200 import ops
-    kw = dict(graph.cfg.solver.optim.args)
-    graph.flat_grads = train.FlatState(graph.optimizer.param_groups, graph._base_lrs, betas=tuple(kw.get("betas", (0.9, 0.999))),
-                                       eps=float(kw.get("eps", 1e-8)), max_norm=graph.grad_norm)
-    graph.flat_grads.lr_factor.fill_(graph._lr_lambda(0))
-    train.register_packs(graph.module, graph.flat_grads)
+    graph._make_flat_state()
     graph._raw_step()
     ops.clear_shadows()
     worst = (1.0, None)

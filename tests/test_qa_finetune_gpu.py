@@ -487,7 +487,7 @@ def test_qa_graph_replay_reads_new_batch(config):
 def test_qa_graph_step_matches_eager_step_parameters(config):
     """One step through the captured path's flat state (what the graph records) moves every parameter like the eager step:
     same sign on the coordinates whose gradient is far above the bf16 noise, and the same mean step size."""
-    from sceneverse_b200 import ops, train
+    from sceneverse_b200 import ops
     batch = _qa_batch(config, 9)
     eager, graph = _qa_step(config, False), _qa_step(config, True)
     graph.module.load_state_dict(eager.module.state_dict())
@@ -496,11 +496,7 @@ def test_qa_graph_step_matches_eager_step_parameters(config):
     graph._probe_unused(dict(batch))
     eager.step(dict(batch))
     graph.static_batch = {k: v.clone() for k, v in batch.items()}
-    kw = dict(graph.cfg.solver.optim.args)
-    graph.flat_grads = train.FlatState(graph.optimizer.param_groups, graph._base_lrs, betas=tuple(kw.get("betas", (0.9, 0.999))),
-                                       eps=float(kw.get("eps", 1e-8)), max_norm=graph.grad_norm)
-    graph.flat_grads.lr_factor.fill_(graph._lr_lambda(0))
-    train.register_packs(graph.module, graph.flat_grads)
+    graph._make_flat_state()
     graph._raw_step()
     ops.clear_shadows()
     worst, checked, qa = (1.0, None), 0, 0
