@@ -115,6 +115,11 @@ int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const
                                   void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w, float *dvec, float dropout_p,
                                   unsigned long long seed, void *stream);
 
+/* Both attention directions skip every 64-key block whose keys are all masked (key_padding_mask or past Lk): such a block
+ * only adds zero weights, so the results are the full sweep's bit for bit, up to the sign of a zero.  Tests: on = 1 makes
+ * every launch sweep all blocks again, on = 0 (default) restores skipping. */
+int sv_attention_visit_all_blocks(int on);
+
 /* Fused dropout + residual add + LayerNorm:  y = LayerNorm(residual + dropout(x)) * gamma + beta  (reference: the post-norm
  * blocks of modules/layers/transformers.py:145-154,311-315; plain LayerNorm of modules/utils.py:18-25 with residual = NULL,
  * dropout_p = 0).  x, residual, y, s: (R,D) contiguous, bf16 (io_bf16 = 1) or f32; D % 8 == 0, D <= 1024; gamma, beta (D)

@@ -35,6 +35,7 @@ struct FwdArgs {
   float inv_keep;
   unsigned long long seed;
   const unsigned long long *seed_offset;  // device counter added to the seed at run time (or null)
+  int all_blocks;                  // 1 = visit every key block (sv_attention_visit_all_blocks)
 };
 
 template <bool GATED, bool DROP>
@@ -53,6 +54,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
   uint8_t *sP = sV + NK64 * 128;             // 2 x [8][64][8] K-major, no swizzle: P of the even / odd key blocks
   float *kb = reinterpret_cast<float *>(sP + 16384);        // [nblk * 64] additive key bias: 0 or -inf
   uint64_t *bar = reinterpret_cast<uint64_t *>(kb + 384);  // Q, K and V landed
+  uint32_t *wlive = reinterpret_cast<uint32_t *>(bar + 1);  // [4] per warp: bit blk = key block blk holds a live key
 
   const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
   const int rl = w * 16 + (lane >> 2);             // this thread's first row in the tile (second: rl + 8)
@@ -67,15 +69,25 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
   }
   // V rows [NK, NK64) are never written by TMA: zero them so that the P V terms of the padded keys are exact zeros
   for (int i = tid; i < (NK64 - NK) * 8; i += 128) reinterpret_cast<uint4 *>(sV + NK * 128)[i] = make_uint4(0, 0, 0, 0);
-  for (int j = tid; j < NK64; j += 128)
-    kb[j] = (j < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + j])) ? 0.f : -INFINITY;
+  uint32_t lm = 0u;
+  for (int j = tid; j < NK64; j += 128) {
+    const bool live = j < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + j]);
+    kb[j] = live ? 0.f : -INFINITY;
+    lm |= (uint32_t)live << (j >> 6);
+  }
+  lm = __reduce_or_sync(0xffffffffu, lm);
+  if (lane == 0) wlive[w] = lm;
   fence_proxy_async_smem();
   __syncthreads();
+  // the key blocks visited: those holding a live key (attn_common.cuh, block skipping); K / V are loaded up to the last
+  const uint32_t live = a.all_blocks ? (1u << nblk) - 1u : wlive[0] | wlive[1] | wlive[2] | wlive[3];
+  const int nlive = __popc(live);
+  const int kvbox = live ? min(nkbox, 4 * (32 - __clz(live))) : 0;
   if (tid == 0) {
-    mbar_expect_tx(bar, rows_bytes(q0, 4, a.Lq) + 2 * rows_bytes(0, nkbox, a.Lk));
+    mbar_expect_tx(bar, rows_bytes(q0, 4, a.Lq) + 2 * rows_bytes(0, kvbox, a.Lk));
     tma_rows(sQ, &mq, h, q0, 4, a.Lq, b, bar);
-    tma_rows(sK, &mk, h, 0, nkbox, a.Lk, b, bar);
-    tma_rows(sV, &mv, h, 0, nkbox, a.Lk, b, bar);
+    tma_rows(sK, &mk, h, 0, kvbox, a.Lk, b, bar);
+    tma_rows(sV, &mv, h, 0, kvbox, a.Lk, b, bar);
   }
   const float c2 = a.scale * LOG2E;
   const uint32_t aQ = smem_u32(sQ), aK = smem_u32(sK), aV = smem_u32(sV), aP = smem_u32(sP);
@@ -120,7 +132,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
         m2[r] = fmaxf(m2[r], fmaxf(fmaf(s[4 * j + 2 * r], c2, k2.x), fmaf(s[4 * j + 2 * r + 1], c2, k2.y)));
     }
   };
-  for (int blk = 0; blk < nblk; ++blk) {
+  for (int it = 0; it < nlive; ++it) {
+    const int blk = nth_block(live, it);
     s_block(s, blk);
     row_max(blk);
   }
@@ -133,13 +146,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
 
   // ---- pass 2: p = 2^(x - max), row sum, dropout, bf16 P block, O += P V -------------------------------------------------
   float sum[2] = {0.f, 0.f};
-  float o[32];
-  for (int blk = 0; blk < nblk; ++blk) {
-    const int n = block_cols(blk, NK);
-    // completes the P V chain of block blk - 1 too; every warp passed its wait for the chain of block blk - 2 before the
-    // barrier that ended block blk - 1, so this block's P buffer is free
+  float o[32];   // written by wgmma only; never read when no block is visited
+  for (int it = 0; it < nlive; ++it) {
+    const int blk = nth_block(live, it), n = block_cols(blk, NK);
+    // completes the P V chain of visited block it - 1 too; every warp passed its wait for the chain of block it - 2
+    // before the barrier that ended block it - 1, so this block's P buffer is free
     s_block(s, blk);
-    uint8_t *P = sP + (blk & 1) * 8192;
+    uint8_t *P = sP + (it & 1) * 8192;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       if (8 * j >= n) {   // keys past NK: zero weights (the P V chain runs over the whole block)
@@ -178,7 +191,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
     wgmma_fence();
     // V staged once, read MN-major; all four k16 steps (a chain cut short at the last block makes ptxas serialize it);
     // left in flight behind the next S chain
-    mma_gc(o, aP + (blk & 1) * 8192, aV + blk * 8192, 64, blk > 0);
+    mma_gc(o, aP + (it & 1) * 8192, aV + blk * 8192, 64, it > 0);
     wgmma_commit();
   }
   wgmma_wait<0>();
@@ -197,16 +210,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
       a.lse[((size_t)b * a.H + h) * a.Lq + qi[r]] = tot > 0.f ? (m2[r] + lg2f(tot)) * LN2 : INFINITY;
     __nv_bfloat16 *op = a.out + (size_t)b * a.o_bs + (size_t)qi[r] * a.o_rs + h * DH + cq;
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      *reinterpret_cast<uint32_t *>(op + 8 * j) = pack_bf16(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
+    for (int j = 0; j < 8; ++j)   // every key masked (no block visited): output row 0
+      *reinterpret_cast<uint32_t *>(op + 8 * j) =
+          nlive == 0 ? 0u : pack_bf16(o[4 * j + 2 * r] * inv, o[4 * j + 2 * r + 1] * inv);
   }
 }
 
 template <bool GATED, bool DROP>
 int launch_fwd(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &mv, const FwdArgs &a, cudaStream_t st) {
   const int NK = (a.Lk + 15) & ~15, NK64 = (a.Lk + 63) & ~63;
-  const size_t smem = 1024 + 8192 + (size_t)(NK + NK64) * 128 + 16384 + 384 * 4 + 8;
-  constexpr size_t SMEM_MAX = 1024 + 8192 + 384 * 128 * 2 + 16384 + 384 * 4 + 8;
+  const size_t smem = 1024 + 8192 + (size_t)(NK + NK64) * 128 + 16384 + 384 * 4 + 8 + 16;
+  constexpr size_t SMEM_MAX = 1024 + 8192 + 384 * 128 * 2 + 16384 + 384 * 4 + 8 + 16;
   auto kern = attn_fwd_kernel<GATED, DROP>;
   static bool configured[64] = {false};
   int dev = 0;
@@ -223,6 +237,13 @@ int launch_fwd(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap &
 }
 
 }  // namespace
+
+int attn::g_visit_all_blocks = 0;
+
+extern "C" int sv_attention_visit_all_blocks(int on) {
+  attn::g_visit_all_blocks = on ? 1 : 0;
+  return SV_OK;
+}
 
 extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
                                              int k_rs, const void *v, long long v_bs, int v_rs, void *out, long long o_bs,
@@ -249,6 +270,7 @@ extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int 
   a.t16 = drop_threshold(dropout_p);
   a.inv_keep = 1.0f / (1.0f - dropout_p);
   a.seed = seed; a.seed_offset = sv::g_seed_offset;
+  a.all_blocks = g_visit_all_blocks;
   CUtensorMap mq, mk, mv;
   int rc = make_map(&mq, q, B, Lq, H, q_rs, q_bs);
   if (rc) return rc;

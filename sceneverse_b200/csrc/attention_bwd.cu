@@ -30,6 +30,7 @@ struct BwdArgs {
   float inv_keep;
   unsigned long long seed;
   const unsigned long long *seed_offset;  // device counter added to the seed at run time (or null)
+  int all_blocks;                    // 1 = no block skipping (sv_attention_visit_all_blocks)
 };
 
 // 64 columns of a row from the accumulator fragment (row r_lo + 8 r) -> bf16 row of `dst`
@@ -37,13 +38,18 @@ __device__ __forceinline__ void store_row_frag(const float (&d)[32], int r, __nv
 #pragma unroll
   for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t *>(dst + 8 * j + cq) = pack_bf16(d[4 * j + 2 * r], d[4 * j + 2 * r + 1]);
 }
+// this thread's 16 columns of a zero row
+__device__ __forceinline__ void store_row_zero(__nv_bfloat16 *dst, int cq) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t *>(dst + 8 * j + cq) = 0u;
+}
 
 constexpr int BWD_STAGES = 2;   // column-block ring: block j + 1 lands while block j is processed
 
 template <int SIDE>
 constexpr size_t bwd_smem_bytes(int NC, bool gated) {
   return 1024 + 16384 + (size_t)BWD_STAGES * 16384 + (SIDE == 1 ? 16384 : 8192) +
-         (size_t)(SIDE == 0 ? NC : (gated ? 9 : 3) * NC) * 4 + 8 * (BWD_STAGES + 1);
+         (size_t)(SIDE == 0 ? NC : (gated ? 9 : 3) * NC) * 4 + 8 * (BWD_STAGES + 1) + 16;
 }
 
 // One CTA = one warpgroup = one unit (scene, head, 64 rows of the row operand), CTAs ordered by (scene, head) first so
@@ -73,6 +79,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
   float *Ws = vec + 3 * NC;
   // barriers [0, BWD_STAGES): column block landed in that buffer, BWD_STAGES: row tile landed
   uint64_t *bars = reinterpret_cast<uint64_t *>(vec + (SIDE == 0 ? NC : (GATED ? 9 : 3) * NC));
+  // [4] per warp: SIDE 0: bit blk = key block blk holds a live key; SIDE 1: one of the tile's keys is live
+  uint32_t *wlive = reinterpret_cast<uint32_t *>(bars + BWD_STAGES + 1);
 
   const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31;
   const int rl = w * 16 + (lane >> 2);             // this thread's first row in the tile (second: rl + 8)
@@ -82,8 +90,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
   const int b = bh / a.H, h = bh % a.H;
   const int E = a.H * DH;
   const int nblk = (NC + 63) >> 6;
-  auto load_cblock = [&](int blk) {
-    const int buf = blk % BWD_STAGES;
+  uint32_t live = 0u;   // the column blocks visited (attn_common.cuh, block skipping)
+  // column block blk, the i-th visited one -> ring buffer i % BWD_STAGES
+  auto load_cblock = [&](int i, int blk) {
+    const int buf = i % BWD_STAGES;
     mbar_expect_tx(&bars[buf], 2 * rows_bytes(blk * 64, 4, Lc));
     tma_rows(sC + buf * 16384, &mC1, h, blk * 64, 4, Lc, b, &bars[buf]);
     tma_rows(sC + buf * 16384 + 8192, &mC2, h, blk * 64, 4, Lc, b, &bars[buf]);
@@ -102,9 +112,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
   // values.  Column-block rows past the last box only reach S / dP columns the element-wise stage never reads.
   for (int i = tid; i < 16384 / 16; i += 128) reinterpret_cast<uint4 *>(smem)[i] = make_uint4(0, 0, 0, 0);
   // per-column vectors
+  uint32_t lm = 0u;
+  if (SIDE == 1 && tid < 64) lm = r0 + tid < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + r0 + tid]);
   for (int c = tid; c < NC; c += 128) {
     if (SIDE == 0) {
-      kb[c] = (c < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + c])) ? 0.f : -INFINITY;
+      const bool lc = c < a.Lk && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + c]);
+      kb[c] = lc ? 0.f : -INFINITY;
+      lm |= (uint32_t)lc << (c >> 6);
     } else {
       const bool live = c < a.Lq;
       const size_t r = ((size_t)b * a.H + h) * a.Lq + c;
@@ -118,13 +132,18 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
       }
     }
   }
+  lm = __reduce_or_sync(0xffffffffu, lm);
+  if (lane == 0) wlive[w] = lm;
   fence_proxy_async_smem();
   __syncthreads();
-  if (tid == 0) {
+  live = wlive[0] | wlive[1] | wlive[2] | wlive[3];
+  if (a.all_blocks || (SIDE == 1 && live)) live = (1u << nblk) - 1u;
+  const int nlive = __popc(live);
+  if (tid == 0 && nlive > 0) {
     mbar_expect_tx(&bars[BWD_STAGES], 2 * rows_bytes(r0, 4, Lr));
     tma_rows(sR1, &mR1, h, r0, 4, Lr, b, &bars[BWD_STAGES]);
     tma_rows(sR2, &mR2, h, r0, 4, Lr, b, &bars[BWD_STAGES]);
-    for (int i = 0; i < BWD_STAGES - 1 && i < nblk; ++i) load_cblock(i);
+    for (int i = 0; i < BWD_STAGES - 1 && i < nlive; ++i) load_cblock(i, nth_block(live, i));
   }
   const float c2 = a.scale * LOG2E;
   const uint32_t aR1 = smem_u32(sR1), aR2 = smem_u32(sR2);
@@ -175,12 +194,37 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
       klive[r] = rlive[r] && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + ri[r]]);
     }
   }
+  if (nlive == 0) {
+    // SIDE 0: every key masked (dQ and the gate-weight gradients are 0); SIDE 1: every key of the tile masked (dK = dV
+    // = 0).  Nothing was loaded.  (The accumulators below are only ever written by wgmma: defining them here would
+    // serialize the chains.)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      if (!rlive[r]) continue;
+      if (SIDE == 0) {
+        store_row_zero(a.dq + ((size_t)b * a.Lq + ri[r]) * a.d_rs + h * DH, cq);
+        if (GATED && (lane & 3) == 0 && a.dsw != nullptr) {
+          float *g = a.dsw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6;
+#pragma unroll
+          for (int k = 0; k < 6; ++k) g[k] = 0.f;
+        }
+      } else {
+        store_row_zero(a.dk + ((size_t)b * a.Lk + ri[r]) * a.d_rs + h * DH, cq);
+        store_row_zero(a.dv + ((size_t)b * a.Lk + ri[r]) * a.d_rs + h * DH, cq);
+      }
+    }
+    return;
+  }
   mbar_wait(&bars[BWD_STAGES], 0);
 
   float o1[32], o2[32];
-  for (int blk = 0; blk < nblk; ++blk) {
-    const int buf = blk % BWD_STAGES, n = block_cols(blk, NC);
-    mbar_wait(&bars[buf], (uint32_t)(blk / BWD_STAGES) & 1u);
+  int it = 0;
+  do {
+    const int blk = nth_block(live, it), buf = it % BWD_STAGES;
+    // n is CTA-uniform; the shuffle lets ptxas see that too (a width it takes for divergent serializes the output chains)
+    const int n = __shfl_sync(0xffffffffu, block_cols(blk, NC), 0);
+    const int pre = nth_block(live, it + BWD_STAGES - 1);   // the block loaded once this one's S / dP are done, or -1
+    mbar_wait(&bars[buf], (uint32_t)(it / BWD_STAGES) & 1u);
     const uint32_t aC1 = smem_u32(sC) + buf * 16384, aC2 = aC1 + 8192;
     // ---- S_blk, dP_blk (queued behind the previous block's output chains) ---------------------------------------------
     float sa[32], dp[32];
@@ -191,9 +235,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
     wgmma_wait<0>();
     fence_regs(sa);
     fence_regs(dp);
-    // every warp's chains are complete: the buffer of block blk - 1 and the dS / P tiles are free
+    // every warp's chains are complete: the buffer of visited block it - 1 and the dS / P tiles are free
     __syncthreads();
-    if (tid == 0 && blk + BWD_STAGES - 1 < nblk) load_cblock(blk + BWD_STAGES - 1);
+    if (tid == 0 && pre >= 0) load_cblock(it + BWD_STAGES - 1, pre);
 
     // ---- element-wise stage over this thread's fragment: rows rl + 8 r, columns 8 j + cq + e of the block ------------
 #pragma unroll
@@ -263,10 +307,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
 
     // ---- accumulate the outputs over this block's columns (column operand read MN-major), left in flight ---------------
     wgmma_fence();
-    mma_gc(o1, aG1, aC1, n, blk > 0);
-    if (SIDE == 1) mma_gc(o2, aG2, aC2, n, blk > 0);
+    mma_gc(o1, aG1, aC1, n, it > 0);
+    if (SIDE == 1) mma_gc(o2, aG2, aC2, n, it > 0);
     wgmma_commit();
-  }
+  } while (++it < nlive);
   wgmma_wait<0>();
   fence_regs(o1);
   if (SIDE == 1) fence_regs(o2);
@@ -357,6 +401,7 @@ extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int 
   a.t16 = drop_threshold(dropout_p);
   a.inv_keep = 1.0f / (1.0f - dropout_p);
   a.seed = seed; a.seed_offset = sv::g_seed_offset;
+  a.all_blocks = attn::g_visit_all_blocks;
   CUtensorMap mq, mk, mv, mo;
   int rc = make_map(&mq, q, B, Lq, H, q_rs, q_bs);
   if (rc) return rc;

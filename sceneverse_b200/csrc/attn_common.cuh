@@ -15,6 +15,13 @@
 // element-wise work and the backward's output chains of the last block stop at the column count rounded up to 16 (the
 // TMA box and the k16 step).  Every output element keeps the chain of k16 steps it had with whole 64-column blocks: the
 // skipped steps only ever added products with exact zeros.
+//
+// Block skipping: a 64-key block in which every key is masked (key-padding mask or past Lk) is never visited — its
+// logits are all -inf, so it only ever added P = 0 and dS = 0 products and -inf to the row maximum.  The forward and the
+// backward's query-row pass sweep the live key blocks only (the forward loads K / V up to the last live one), and a
+// key-row unit of the backward whose 64 keys are all masked writes zero dK / dV rows without loading anything.  The
+// visited blocks keep their order and their chains, so every result is bit-for-bit the one of the full sweep, up to the
+// sign of a zero.  sv_attention_visit_all_blocks(1) switches skipping off (tests compare both paths).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -83,6 +90,11 @@ struct GateW {
 };
 
 // ---- wgmma chains of one 64-row unit -----------------------------------------------------------------------------------
+// index of the i-th set bit of `live` (the i-th visited column block), -1 past the last
+__device__ __forceinline__ int nth_block(uint32_t live, int i) {
+  for (; i > 0 && live; --i) live &= live - 1u;
+  return live ? __ffs(live) - 1 : -1;
+}
 // width of column block `blk` of a sweep over `n16` columns (a multiple of 16): 64, the last one 16, 32, 48 or 64
 __device__ __forceinline__ int block_cols(int blk, int n16) {
   const int rest = n16 - blk * 64;
@@ -165,6 +177,9 @@ inline int make_map(CUtensorMap *map, const void *ptr, int B, int L, int H, int 
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? SV_OK : SV_ERR_INVALID_ARG;
 }
+// sv_attention_visit_all_blocks: 1 = sweep every key block and run every key-row unit (no block skipping)
+extern int g_visit_all_blocks;
+
 inline uint32_t drop_threshold(float p) {
   if (!(p > 0.f)) return 0u;
   unsigned t = (unsigned)((double)p * 65536.0 + 0.5);

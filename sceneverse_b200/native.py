@@ -196,6 +196,11 @@ def embedding_bwd(grad_out, ids, dw, padding_idx=-1):
     return dw
 
 
+def attention_visit_all_blocks(on):
+    """1 = the attention kernels sweep every key block, 0 (default) = skip the fully masked ones (svgps.h)."""
+    _lib.check(_lib.gps(), _lib.gps().sv_attention_visit_all_blocks(int(on)), "sv_attention_visit_all_blocks")
+
+
 def gemm_force_ctas(n):
     """0 = heuristic, 1 / 2 / 4 = tiles of 64 / 128 / 192 output columns; bits 8.. are timing-only profiling switches
     (svgps.h)."""

@@ -34,6 +34,20 @@ for name, L, masked, gated, p in STEP:
     res[f"{name}_fwd"] = t(lambda: native.attention(q, k, v, H, return_lse=True, **fkw), n=100)
     out, lse = native.attention(q, k, v, H, return_lse=True, **fkw)
     res[f"{name}_bwd"] = t(lambda: native.attention_backward(q, k, v, out, go, lse, H, **bkw), n=100)
+# block skipping (csrc/attn_common.cuh) at the scene-caption shape: captions of 8..300 tokens, the length distribution of
+# synthetic.scene_batch, with every fully masked key block skipped (default) against every block visited; alternated
+q, k, v, go = (rnd(B, 300, E).bfloat16() for _ in range(4))
+lens = torch.randint(8, 301, (B,), device="cuda", generator=g)
+cap = dict(key_padding_mask=torch.arange(300, device="cuda")[None] >= lens[:, None], dropout_p=0.1, seed=5)
+for rep in range(1 if quick else 3):
+    for tag, visit_all in (("skip", 0), ("all", 1)):
+        native.attention_visit_all_blocks(visit_all)
+        f = t(lambda: native.attention(q, k, v, H, return_lse=True, **cap), n=100)
+        out, lse = native.attention(q, k, v, H, return_lse=True, **cap)
+        bw = t(lambda: native.attention_backward(q, k, v, out, go, lse, H, **cap), n=100)
+        for key, val in ((f"bert300_len8to300_{tag}_fwd", f), (f"bert300_len8to300_{tag}_bwd", bw)):
+            res[key] = min(res.get(key, val), val)
+native.attention_visit_all_blocks(0)
 for name, Lq, Lk in [("joint130", 130, 130), ("self80", 80, 80), ("cross80x50", 80, 50)]:
     q = rnd(B, Lq, E).bfloat16(); k = rnd(B, Lk, E).bfloat16(); v = rnd(B, Lk, E).bfloat16(); go = rnd(B, Lq, E).bfloat16()
     for p in (0.0, 0.1):
