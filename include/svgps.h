@@ -158,6 +158,15 @@ int sv_dropout_seed_offset(const unsigned long long *device_counter);
 int sv_colsum(const void *x, long long row_stride, int is_bf16, int R, int N, float *out, float *scratch, void *stream);
 int sv_colsum_scratch_floats(int N);
 
+/* Batched column sums out[b][c] = sum_r x[b][r][c] of B row-major (R, N) matrices batch_stride elements apart (rows
+ * row_stride apart, N % 8 == 0, both strides % 8 == 0), written to a contiguous (B, N) out in x's dtype (is_bf16) after fp32
+ * accumulation in the fixed order of sv_colsum: the backward of the per-scene broadcast (reference:
+ * model/openvocab.py:170-173 `repeat` of the object features over the U utterances of a scene), the U-sum of the (B, U, O*D)
+ * gradient.  scratch: sv_colsum_batched_scratch_floats(B, R, N) floats. */
+int sv_colsum_batched(const void *x, long long row_stride, long long batch_stride, int is_bf16, int B, int R, int N, void *out,
+                      float *scratch, void *stream);
+long long sv_colsum_batched_scratch_floats(int B, int R, int N);
+
 /* calc_pairwise_locs, 'center' relation (reference: modules/utils.py:38-87): centers (B,O,*) f32 with row stride
  * row_stride (>= 3 floats; xyz first) -> out (B,O,O,5) f32 = [dist/max_dist, dz/dist, dist2d/dist, dy/dist2d, dx/dist2d];
  * dist_norm = 0 keeps the raw distance in slot 0.  eps sits inside the square roots (1e-10 in the reference). */

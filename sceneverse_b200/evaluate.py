@@ -8,7 +8,9 @@ several ranks evaluate) and builds the reference's dictionary: integer totals di
 batch-size-weighted average of per-batch ratios, accumulated on the device in the reference's float64 order.
 `counts_to_metrics` turns one batch's counter values into `batch_metrics`; train.PretrainStep's per-step logs use it too.
 
-Not supported (NotImplementedError): `cfg.eval.save` (results.json) and per-scene (3-D) grounding logits.
+Not supported (NotImplementedError): `cfg.eval.save` (results.json).  Per-scene batches (model.OpenVocabPerScene: B scenes x U
+utterances, og3d_logits (B, U, O)) are counted by the grounding evaluators after `flatten_per_scene`, which EvalRunner applies;
+PretrainEval has no per-scene form.
 An item whose `valid` entry is False (the padding of a last partial batch) counts nothing."""
 import math
 
@@ -17,7 +19,8 @@ import torch.distributed as dist
 
 from . import _lib
 
-__all__ = ["ScanReferEval", "ReferIt3DEval", "ScanQAEval", "SQA3DEval", "PretrainObjEval", "PretrainEval", "EvalRunner"]
+__all__ = ["ScanReferEval", "ReferIt3DEval", "ScanQAEval", "SQA3DEval", "PretrainObjEval", "PretrainEval", "EvalRunner",
+           "flatten_per_scene"]
 
 
 def _is_bf16(t):
@@ -57,6 +60,35 @@ def _obj_logit_keys(data_dict):
     shape = data_dict["obj_labels"].shape
     return [k for k, v in data_dict.items() if k.endswith("logits") and torch.is_tensor(v) and v.ndim == 3
             and v.shape[:2] == shape]
+
+
+_PER_SCENE_ITEM_KEYS = ("og3d_logits", "tgt_object_id_iou25", "tgt_object_id_iou50", "is_multiple", "is_hard",
+                        "is_view_dependent")
+
+
+def flatten_per_scene(data_dict):
+    """A per-scene data dict (og3d_logits (B, U, O)) as B*U grounding items, as evaluator/scanrefer_eval.py:15-21 and
+    referit3d_eval.py:15-20 flatten it before counting: og3d_logits, tgt_object_id_iou25 / 50 (B*U, O); is_multiple, is_hard,
+    is_view_dependent (B*U); tgt_object_id, tgt_object_label (B*U, 1).  These are views (safe inside a CUDA graph).  A
+    per-scene `valid` (B) is repeated over U and kept as `scene_valid` for the per-scene object keys (obj_labels, obj_masks
+    and the (B, O, C) object logits), which stay as they are; object logits of B*U rows are not counted.  Duplicate
+    utterances (per_scene_pad fills every scene to U) count like any other.  Returns a new dict; a 2-D batch is returned
+    as a copy."""
+    d = dict(data_dict)
+    og = d["og3d_logits"]
+    if og.dim() != 3:
+        return d
+    B, U = og.shape[:2]
+    for k in _PER_SCENE_ITEM_KEYS:
+        if k in d:
+            d[k] = d[k].flatten(0, 1)
+    for k in ("tgt_object_id", "tgt_object_label"):
+        if k in d:
+            d[k] = d[k].reshape(B * U, 1)
+    if d.get("valid") is not None:
+        d["scene_valid"] = d["valid"]
+        d["valid"] = d["valid"].unsqueeze(1).expand(B, U).reshape(B * U)
+    return d
 
 
 def _launch_obj_cls(tensors, data_dict, valid, counters, split=None):
@@ -155,7 +187,8 @@ class _GroundingEval(_CounterEvaluator):
     def _launch(self, data_dict, valid, counters):
         og = data_dict["og3d_logits"]
         if og.ndim == 3:
-            raise NotImplementedError(f"{type(self).__name__}: per-scene (3-D) og3d_logits are not supported")
+            raise NotImplementedError(f"{type(self).__name__}: per-scene (3-D) og3d_logits are counted after "
+                                      "evaluate.flatten_per_scene(data_dict)")
         if og.dim() != 2:
             raise ValueError(f"og3d_logits must be (B, O), got {tuple(og.shape)}")
         B, O = og.shape
@@ -187,6 +220,8 @@ class _GroundingEval(_CounterEvaluator):
             if self._obj_keys and keys != self._obj_keys:
                 raise ValueError(f"object logits changed between batches: {self._obj_keys} -> {keys}")
             self._obj_keys = keys
+            if "scene_valid" in data_dict:        # flatten_per_scene: the object keys are per scene
+                valid = _bytes(data_dict["scene_valid"])
             _launch_obj_cls([data_dict[k] for k in keys], data_dict, valid, counters[_lib.EVG_OBJ:])
 
     def _obj_metrics(self, c, m):
@@ -373,6 +408,9 @@ class PretrainEval(_CounterEvaluator):
         super().__init__(*a, **k)
 
     def _launch(self, data_dict, valid, counters):
+        if data_dict["masked_lm_labels"].dim() == 3 or ("og3d_logits" in data_dict and data_dict["og3d_logits"].dim() == 3):
+            raise ValueError("PretrainEval has no per-scene form: the per-scene model's B*U logits rows do not match its "
+                             "(B, O) object masks and (B, U) targets")
         lm = data_dict["txt_lm_cls_logits"]
         labels = _i64(data_dict["masked_lm_labels"], "masked_lm_labels")
         if lm.dim() != 3 or lm.stride(2) != 1 or lm.stride(0) != lm.shape[1] * lm.stride(1):
@@ -441,7 +479,8 @@ class EvalRunner:
     it is: the bf16 weight shadows that training keeps current are what the native linears read, so no weight is copied.
     `run(batches)` evaluates an iterable of batches (dicts of device tensors, at most `batch_size` items each; a smaller last
     batch is padded by repeating its first item, with `valid` False for the padding) and returns `record()` of every
-    evaluator.  The model's train / eval mode is restored afterwards; the run writes no parameter and no optimizer state."""
+    evaluator.  With a per-scene model (txt_ids (B, U, T)) an item is a scene: a partial batch is padded by whole scenes and
+    the output goes through `flatten_per_scene` before the evaluators.  The model's train / eval mode is restored afterwards; the run writes no parameter and no optimizer state."""
 
     def __init__(self, forward, evaluators, batch_size, dtype=torch.bfloat16):
         if isinstance(getattr(forward, "module", None), torch.nn.Module) and hasattr(forward.module, "model"):
@@ -461,6 +500,9 @@ class EvalRunner:
         with torch.autocast("cuda", dtype=self.dtype, enabled=self.dtype != torch.float32):
             out = self.forward(dict(batch))
         out["valid"] = batch["valid"]
+        og = out.get("og3d_logits")
+        if og is not None and og.dim() == 3:
+            out = flatten_per_scene(out)          # per-scene model: B scenes x U utterances
         for ev in self.evaluators:
             ev.update(out)
 

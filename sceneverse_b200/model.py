@@ -165,6 +165,90 @@ class OpenVocab(nn.Module):
         return groups
 
 
+# what the reference's OpenVocabPerScene cannot run on a per-scene batch (model/openvocab.py:141-230), and why
+PER_SCENE_UNSUPPORTED = {
+    "og3d_loss": "cross-entropy over the (B, U, O) per-scene logits would treat U as the class axis",
+    "TextSceneBetweenBatch": "the per-scene model sets no scene_embed / scene_text_embed",
+    "answer_loss": "the QA head is given the un-flattened (B, U, T) txt_masks",
+    "qa_head": "the QA head is given the un-flattened (B, U, T) txt_masks",
+}
+
+
+def check_per_scene(cfg):
+    """Raises ValueError naming the first loss or head of `cfg` the per-scene model cannot run."""
+    cfg = to_cfg(cfg)
+    for k in list(cfg.model.get("loss_list", [])) + list(cfg.model.get("vis_loss_list", [])) + \
+            list(cfg.model.heads.head_list):
+        if k in PER_SCENE_UNSUPPORTED:
+            raise ValueError(f"OpenVocabPerScene cannot use {k!r}: {PER_SCENE_UNSUPPORTED[k]}")
+
+
+class OpenVocabPerScene(OpenVocab):
+    """Per-scene grounding (reference: model/openvocab.py:129-255 `OpenVocabPerScene`): the same submodules, parameter names
+    and optimizer groups as OpenVocab, so checkpoints move between the two.  A batch is per-scene when txt_ids is (B, U, T):
+    U utterances about each of B scenes.  The language encoder, V2 and the heads then run on B*U rows, while PointNet++ and
+    the spatial layers run once per scene; their (B, O, D) output (vision dropout applied) is repeated U times by
+    ops.scene_broadcast, whose backward sums the U copies.  og3d_logits is (B, U, O).  The ground head is never called and
+    no scene-caption embedding is made, in either path; a 2-D batch is OpenVocab without those two."""
+
+    def __init__(self, cfg):
+        check_per_scene(cfg)
+        super().__init__(cfg)
+        self.use_scene_cap = False
+
+    def forward(self, data_dict):
+        if data_dict['txt_ids'].dim() != 3:
+            return self._forward(data_dict, None)
+        return self._forward(data_dict, data_dict['txt_ids'].shape[1])
+
+    def _forward(self, data_dict, U):
+        if 'cur_step' not in data_dict:
+            data_dict['cur_step'], data_dict['total_steps'] = 1, 1
+        txt_ids, txt_masks = data_dict['txt_ids'], data_dict['txt_masks']
+        if U is not None:
+            txt_ids, txt_masks = txt_ids.reshape(-1, txt_ids.shape[-1]), txt_masks.reshape(-1, txt_masks.shape[-1])
+        lang = self.lang_encoder(txt_ids, txt_masks)
+        hook = getattr(self, "_lang_grad_hook", None)
+        if hook is not None and lang.requires_grad:
+            lang.register_hook(hook)
+        obj, _, obj_cls_raw = self.point_encoder(data_dict['obj_fts'].float(), data_dict['obj_locs'], data_dict['obj_masks'],
+                                                 data_dict['obj_sem_masks'], data_dict.get('obj_labels'),
+                                                 data_dict['cur_step'], data_dict['total_steps'])
+        obj_locs, obj_masks = data_dict['obj_locs'], data_dict['obj_masks']
+        if U is not None:
+            B, O = obj_masks.shape
+            obj = ops.scene_broadcast(obj, U)      # one tensor into V2 and inter_obj_embeds: one U-sum in the backward
+            obj_locs = obj_locs.unsqueeze(1).expand(B, U, O, obj_locs.shape[-1]).reshape(B * U, O, obj_locs.shape[-1])
+            obj_masks = obj_masks.unsqueeze(1).expand(B, U, O).reshape(B * U, O)
+        if self.cfg.model.inter == "before":
+            data_dict["inter_text_embed"], data_dict["inter_obj_embeds"] = lang[:, 0], obj
+        lang_f, obj_f = self.unified_encoder(lang, txt_masks, obj, obj_locs, obj_masks)
+        if self.cfg.model.inter != "before":
+            data_dict["inter_text_embed"], data_dict["inter_obj_embeds"] = lang_f[:, 0], obj_f
+        data_dict["intra_text_embed"], data_dict["intra_obj_embeds"] = lang_f[:, 0], obj_f
+        data_dict['obj_cls_raw_logits'] = obj_cls_raw
+        og3d = torch.einsum("bod,bd->bo", obj_f, lang_f[:, 0])
+        data_dict['og3d_logits'] = og3d.reshape(-1, U, og3d.shape[-1]) if U is not None else og3d
+        if getattr(self, "pretrain_head", None) is not None:
+            output = self.pretrain_head(lang_f, obj_f)
+            if isinstance(output, tuple):
+                data_dict['txt_lm_cls_logits'], data_dict['obj_cls_post_logits'] = output
+            else:
+                data_dict['txt_lm_cls_logits'] = output
+        return data_dict
+
+
+MODELS = {"OpenVocab": OpenVocab, "OpenVocabPerScene": OpenVocabPerScene}
+
+
+def build_model(cfg):
+    """model/build.py:16-17: the class named by cfg.model.name (OpenVocab when the config names none)."""
+    name = to_cfg(cfg).model.get("name", "OpenVocab")
+    if name not in MODELS:
+        raise KeyError(f"No model named {name!r}; known: {sorted(MODELS)}")
+    return MODELS[name](cfg)
+
+
 def pretrain_config(num_gpu=1, with_obj_between=True, text_features=None):
     """configs/final/all_pretrain.yaml:205-258 (model/solver part), with TextObjBetweenBatch un-commented as in
     BASELINE.json configs[3] ("obj+scene+ref losses")."""
@@ -196,6 +280,17 @@ def pretrain_config(num_gpu=1, with_obj_between=True, text_features=None):
             "loss_list": losses, "vis_loss_list": losses,
         },
     }
+
+
+def per_scene_pretrain_config(num_gpu=1, text_features=None):
+    """pretrain_config as OpenVocabPerScene: the losses the reference can run per scene (lm_cls_loss, TextObjWithinBatch,
+    TextObjBetweenBatch) and no scene captions.  Batches are synthetic.per_scene_batch-shaped (txt_ids (B, U, T))."""
+    cfg = pretrain_config(num_gpu, text_features=text_features)
+    cfg["data"]["args"]["use_scene_cap"] = False
+    cfg["model"]["name"] = "OpenVocabPerScene"
+    losses = ["lm_cls_loss", "TextObjWithinBatch", "TextObjBetweenBatch"]
+    cfg["model"]["loss_list"], cfg["model"]["vis_loss_list"] = list(losses), list(losses)
+    return cfg
 
 
 def scanrefer_config(num_gpu=1, text_features=None):

@@ -29,6 +29,8 @@ def all_gather(tensors):
 
 
 def og3d_loss(data_dict):
+    if data_dict["og3d_logits"].dim() == 3:
+        raise ValueError("og3d_loss has no per-scene form: cross-entropy over (B, U, O) logits would treat U as the class axis")
     return ops.cross_entropy(data_dict["og3d_logits"], data_dict["tgt_object_id"].squeeze(1))
 
 
@@ -64,7 +66,8 @@ def _task(cfg):
 class TextObjWithinBatch(nn.Module):
     """contra_loss.py:11-38.  Default: cross-entropy over the valid objects against one target id (B, 1).  task 'ScanQA':
     masked BCE with logits over all object slots against a multi-hot (B, O) target (several objects, or the masked
-    'no target' placeholder slot), weight = obj_masks, summed and divided by B."""
+    'no target' placeholder slot), weight = obj_masks, summed and divided by B.  Per scene (B*U object rows, (B, O) masks,
+    (B, U) targets): each scene's mask repeated for its U utterances, cross-entropy over the B*U rows."""
 
     def __init__(self, cfg):
         super().__init__()
@@ -75,6 +78,15 @@ class TextObjWithinBatch(nn.Module):
         obj_feats = ops.l2_normalize(data_dict["intra_obj_embeds"])
         text_feats = ops.l2_normalize(data_dict["intra_text_embed"])
         logits = torch.einsum("bod,bd->bo", obj_feats, text_feats)
+        masks = data_dict["obj_masks"]
+        if obj_feats.shape[0] != masks.shape[0]:
+            # per scene (contra_loss.py:24-27): B*U rows against (B, O) masks and (B, U) targets
+            if self.bce:
+                raise ValueError("TextObjWithinBatch(task='ScanQA') has no per-scene form")
+            U = obj_feats.shape[0] // masks.shape[0]
+            masks = masks.unsqueeze(1).expand(masks.shape[0], U, masks.shape[1]).reshape(-1, masks.shape[1])
+            logits = logits.masked_fill(masks.logical_not(), -float('inf'))
+            return F.cross_entropy(logits, data_dict["tgt_object_id"].reshape(-1))
         if self.bce:
             labels = data_dict["tgt_object_id"]
             if labels.dim() != 2 or labels.shape != logits.shape:
@@ -124,6 +136,8 @@ class TextObjBetweenBatch(_SymmetricInfoNCE):
     def forward(self, data_dict):
         labels = data_dict["tgt_object_id"]
         obj_feats = data_dict["inter_obj_embeds"]
+        if obj_feats.shape[0] != labels.shape[0]:
+            labels = labels.reshape(-1, 1)          # per scene (contra_loss.py:55-56): (B, U) -> (B*U, 1)
         tgt = obj_feats[torch.arange(labels.size(0), device=labels.device), labels[:, 0], :]
         return self.info_nce(tgt, data_dict["inter_text_embed"])
 

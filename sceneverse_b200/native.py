@@ -101,6 +101,19 @@ def colsum(x):
     return out
 
 
+def colsum_batched(x):
+    """Column sums of each (R, N) matrix of a (B, R, N) bf16 / f32 tensor (rows and matrices may be strided) -> (B, N) in x's
+    dtype, fp32 accumulation in a fixed order; deterministic native kernel."""
+    assert x.is_cuda and x.dim() == 3 and x.stride(2) == 1 and x.dtype in (torch.bfloat16, torch.float32)
+    B, R, N = x.shape
+    lib = _lib.gps()
+    out = torch.empty((B, N), dtype=x.dtype, device=x.device)
+    scratch = torch.empty(lib.sv_colsum_batched_scratch_floats(B, R, N), dtype=torch.float32, device=x.device)
+    _lib.call(lib, "sv_colsum_batched", x.device, x.data_ptr(), x.stride(1), x.stride(0), 1 if x.dtype == torch.bfloat16 else 0,
+              B, R, N, out.data_ptr(), scratch.data_ptr())
+    return out
+
+
 def gemm_ex(a, b, a_transposed=False, b_transposed=False, bias=None, act=None, out_dtype=torch.bfloat16):
     """epilogue(A . B^T) with operands optionally given transposed in memory (no copies):
     a: (M,K), or (K,M) when a_transposed;  b: (N,K), or (K,N) when b_transposed.  bf16 in, bf16 / f32 out (M,N)."""

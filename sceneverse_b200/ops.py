@@ -16,7 +16,8 @@ NATIVE = {"linear": True,               # every nn.Linear: native wgmma GEMM for
           "layer_norm": True,           # dropout + residual add + LayerNorm: one native pass per direction
           "l2_normalize": True,         # F.normalize of the contrastive heads: one native kernel per direction
           "bce_with_logits": True,      # QA answer loss / ScanQA within-batch loss: fused native forward+gradient
-          "attention_pool": True}       # AttFlat pooling of the QA head (one glimpse): one native kernel per direction
+          "attention_pool": True,       # AttFlat pooling of the QA head (one glimpse): one native kernel per direction
+          "scene_broadcast": True}      # per-scene object features over U utterances: native U-sum backward
 
 
 _dropout_calls = [0]
@@ -850,3 +851,36 @@ def cross_entropy(logits, labels, ignore_index=-100):
         if l2.stride(1) == 1:
             return _CrossEntropyFn.apply(l2, labels.reshape(-1).contiguous(), ignore_index, 0)
     return F.cross_entropy(logits.reshape(-1, V).float(), labels.reshape(-1), ignore_index=ignore_index)
+
+
+class _SceneBroadcastFn(torch.autograd.Function):
+    """(B, O, D) -> (B*U, O, D): forward one expand copy, backward the sum over the U copies of each scene
+    (csrc/colsum.cu sv_colsum_batched: fp32 accumulation in a fixed order, written in the gradient's dtype)."""
+
+    @staticmethod
+    def forward(ctx, x, U):
+        B = x.shape[0]
+        ctx.shape = (B, int(U)) + tuple(x.shape[1:])
+        return x.unsqueeze(1).expand(ctx.shape).reshape((B * U,) + tuple(x.shape[1:]))
+
+    @staticmethod
+    def backward(ctx, g):
+        from . import native
+        B, U = ctx.shape[:2]
+        rest = ctx.shape[2:]
+        g3 = g.reshape(B, U, -1).contiguous()
+        if g3.dtype not in (torch.bfloat16, torch.float32):
+            g3 = g3.float()
+        elif g3.data_ptr() % 16:
+            g3 = g3.clone()
+        return native.colsum_batched(g3).view((B,) + rest).to(g.dtype), None
+
+
+def scene_broadcast(x, U):
+    """The per-scene repeat of model/openvocab.py:170-173 (reference): (B, O, D) object features -> (B*U, O, D), every scene's
+    rows repeated for its U utterances (row b*U + u = x[b]).  CUDA: the gradient is summed over U by one native reduction;
+    otherwise torch.  A tensor that needs no gradient can be expanded as a view instead."""
+    if x.is_cuda:
+        return _SceneBroadcastFn.apply(x, int(U))
+    B = x.shape[0]
+    return x.unsqueeze(1).expand((B, int(U)) + tuple(x.shape[1:])).reshape((B * int(U),) + tuple(x.shape[1:]))

@@ -156,3 +156,44 @@ def qa_batch(seed, task="ScanQA", B=32, O=80, P=1024, L=50, Ls=300, num_answers=
                 tgt[b, rng.choice(n, size=int(rng.integers(1, min(3, n) + 1)), replace=False)] = 1
         d["tgt_object_id"] = tgt
     return d
+
+
+def per_scene_batch(seed, B=4, U=64, O=80, P=1024, T=50, min_obj=8):
+    """A per-scene batch (model.OpenVocabPerScene; reference data/data_utils.py:12 `per_scene_pad`): the object keys of
+    scene_batch for B scenes (obj_fts, obj_locs, obj_masks, obj_sem_masks, obj_labels), and U utterances per scene drawn
+    from a separate RNG stream: txt_ids / txt_masks / masked_lm_labels (B, U, T) int64; tgt_object_id and
+    tgt_object_label (B, U) int64, each target a valid object of its scene; is_multiple / is_hard / is_view_dependent (B, U)
+    bool; tgt_object_id_iou25 / tgt_object_id_iou50 (B, U, O) int64 over the valid objects, the target among them, the
+    IoU-50 set inside the IoU-25 set."""
+    s = scene_batch(seed, B=B, O=O, P=P, L=8, Ls=8, min_obj=min_obj)
+    d = {k: s[k] for k in ("obj_fts", "obj_locs", "obj_masks", "obj_sem_masks", "obj_labels")}
+    rng = np.random.default_rng([seed, 0x5CE])
+    n_obj = d["obj_masks"].sum(1)
+    ids = np.zeros((B, U, T), np.int64)
+    masks = np.zeros((B, U, T), np.int64)
+    ell = rng.integers(min(8, T), T + 1, size=(B, U))
+    for b in range(B):
+        for u in range(U):
+            e = int(ell[b, u])
+            ids[b, u, :e] = rng.integers(1000, 30000, size=e)
+            ids[b, u, 0], ids[b, u, e - 1] = 101, 102
+            masks[b, u, :e] = 1
+    d["txt_ids"], d["txt_masks"] = ids, masks
+    lm = np.full((B, U, T), -1, np.int64)
+    pick = (rng.random((B, U, T)) < 0.15) & (masks == 1)
+    pick[:, :, 1] = True  # at least one supervised position per utterance
+    lm[pick] = ids[pick]
+    d["masked_lm_labels"] = lm
+    tgt = np.stack([rng.integers(0, int(n), size=U) for n in n_obj]).astype(np.int64)
+    d["tgt_object_id"] = tgt
+    d["tgt_object_label"] = np.take_along_axis(d["obj_labels"], tgt, 1)
+    valid = d["obj_masks"][:, None, :]
+    iou25 = (rng.random((B, U, O)) < 0.2) & valid
+    iou50 = iou25 & (rng.random((B, U, O)) < 0.6)
+    np.put_along_axis(iou25, tgt[:, :, None], True, 2)
+    np.put_along_axis(iou50, tgt[:, :, None], True, 2)
+    d["tgt_object_id_iou25"], d["tgt_object_id_iou50"] = iou25.astype(np.int64), iou50.astype(np.int64)
+    d["is_multiple"] = rng.random((B, U)) < 0.5
+    d["is_hard"] = rng.random((B, U)) < 0.4
+    d["is_view_dependent"] = rng.random((B, U)) < 0.3
+    return d

@@ -23,7 +23,7 @@ class StepModule(nn.Module):
 
     def __init__(self, cfg):
         super().__init__()
-        self.model = M.OpenVocab(cfg)
+        self.model = M.build_model(cfg)
         c = M.to_cfg(cfg)
         self.loss = L.Loss(c.model.loss_list, c.model.vis_loss_list, num_gpu=c.num_gpu,
                            emulate_dist=bool(c.get("emulate_dist", False)), task=c.get("task"))
@@ -207,6 +207,9 @@ class PretrainStep(CapturedStep):
         than that between two `logs()` calls raise.  None (the default) leaves the step as it is without logs."""
         torch.manual_seed(seed)
         self.cfg = M.to_cfg(cfg)
+        if train_eval is not None and self.cfg.model.get("name") == "OpenVocabPerScene":
+            raise ValueError("PretrainStep(train_eval=...) does not log per-scene steps: OpenVocabPerScene's outputs are "
+                             "B*U rows against (B, U) targets")
         self.device = torch.device(device)
         self.module = StepModule(cfg).to(self.device)
         self.dtype = dtype
