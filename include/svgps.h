@@ -100,13 +100,22 @@ int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const
                                   const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
                                   const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, float *lse,
                                   float dropout_p, unsigned long long seed, void *stream);
+/* The same attention for queries that are the first Lq rows of a sequence of seq_rows (>= Lq) rows, e.g. q = the first
+ * row of each scene of a packed (B, seq_rows, 3E) projection, k / v all of its rows: query i of (b, h) draws the dropout
+ * mask of row (b H + h) seq_rows + i, exactly the mask it has in the launch over all seq_rows queries.
+ * sv_attention_fwd_dropout_bf16 is this call with seq_rows = Lq. */
+int sv_attention_fwd_rows_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                               const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
+                               const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
+                               const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, float *lse,
+                               float dropout_p, unsigned long long seed, int seq_rows, void *stream);
 
 /* Backward of the fused attention (one wgmma kernel template launched twice: dQ + gate-weight gradients with tile rows
  * == queries, dK/dV with tile rows == keys; both recompute P from Q, K, the gate and lse).  q/k/v, dropout_p and seed as in
  * the forward; o, d_o (B,Lq,H*64) bf16 contiguous; dq (B,Lq,*), dk, dv (B,Lk,*) bf16 with rows d_rs (>= H*64) elements
  * apart (scene stride L * d_rs): d_rs = H*64 gives contiguous gradients, d_rs = 3E lets the three be the column slices
  * [0,E) [E,2E) [2E,3E) of ONE packed (B,L,3E) buffer — the gradient of a packed QKV projection, consumed by a single
- * dgrad / wgrad GEMM (requires Lq == Lk).  d_spatial_w (B,Lq,H*6) f32 (NULL without gate; gate requires
+ * dgrad / wgrad GEMM (requires Lq == Lk; see sv_attention_bwd_rows_bf16 otherwise).  d_spatial_w (B,Lq,H*6) f32 (NULL without gate; gate requires
  * spatial_heads == H); dvec (B,H,Lq) f32 scratch.  Lq, Lk <= 384. */
 int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
                                   const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
@@ -114,6 +123,16 @@ int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const
                                   const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk, float scale,
                                   void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w, float *dvec, float dropout_p,
                                   unsigned long long seed, void *stream);
+/* Backward of sv_attention_fwd_rows_bf16 (same seq_rows): dq is (B, seq_rows, *) with scene stride seq_rows * d_rs, its
+ * rows [Lq, seq_rows) are written as zeros, and the dropout masks are those of the forward.  With seq_rows = Lk and
+ * d_rs = 3E, dq | dk | dv are the column slices of one packed (B, Lk, 3E) gradient even when only its first Lq rows are
+ * queries.  sv_attention_bwd_strided_bf16 is this call with seq_rows = Lq. */
+int sv_attention_bwd_rows_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                               const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
+                               const unsigned char *key_padding_mask, const float *spatial_w, const float *pairwise_locs,
+                               const float *lse, int B, int H, int Lq, int Lk, float scale, void *dq, void *dk, void *dv,
+                               int d_rs, float *d_spatial_w, float *dvec, float dropout_p, unsigned long long seed,
+                               int seq_rows, void *stream);
 
 /* Both attention directions skip every 64-key block whose keys are all masked (key_padding_mask or past Lk): such a block
  * only adds zero weights, so the results are the full sweep's bit for bit, up to the sign of a zero.  Tests: on = 1 makes
@@ -136,6 +155,15 @@ int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf16, int R, i
 int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma, const float *mean,
                           const float *rstd, float dropout_p, unsigned long long seed, void *ds, void *dx, float *dgamma,
                           float *dbeta, int accumulate, float *scratch, void *stream);
+/* The same two calls for rows taken every row_key_stride (>= 1) rows of a larger tensor: row r draws the dropout mask of
+ * row r * row_key_stride, so LayerNorm over the first token of each of B sequences of L tokens (R = B, row_key_stride = L)
+ * drops exactly what the call over all B * L rows drops there.  The calls above are these with row_key_stride = 1. */
+int sv_layer_norm_fwd_rows(const void *x, const void *residual, int io_bf16, int R, int D, const float *gamma,
+                           const float *beta, float eps, float dropout_p, unsigned long long seed, void *y, void *s,
+                           float *mean, float *rstd, int row_key_stride, void *stream);
+int sv_layer_norm_bwd_rows(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma, const float *mean,
+                           const float *rstd, float dropout_p, unsigned long long seed, void *ds, void *dx, float *dgamma,
+                           float *dbeta, int accumulate, float *scratch, int row_key_stride, void *stream);
 
 /* Row-wise L2 normalisation y = x / max(||x||_2, eps) over the last dimension and its backward
  * dx = (g - y (y . g)) / ||x|| (rows with ||x|| < eps: g / eps) — F.normalize(x, dim=-1, p=2) of the contrastive heads

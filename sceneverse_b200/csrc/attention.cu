@@ -36,6 +36,7 @@ struct FwdArgs {
   unsigned long long seed;
   const unsigned long long *seed_offset;  // device counter added to the seed at run time (or null)
   int all_blocks;                  // 1 = visit every key block (sv_attention_visit_all_blocks)
+  int seq_rows;                    // dropout row key of query i: (b H + h) seq_rows + i (the queries are the first Lq rows)
 };
 
 template <bool GATED, bool DROP>
@@ -105,7 +106,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap mq, const __grid_constant__ 
       gw[r].load(a.sw + ((size_t)b * a.Lq + qi[r]) * (a.SH * 6) + (a.SH == 1 ? 0 : h) * 6);
       loc[r] = a.locs + ((size_t)b * a.Lq + qi[r]) * (size_t)a.Lk * 5;
     }
-    if (DROP) rk[r] = drop_row_key(seed, ((unsigned long long)b * a.H + h) * a.Lq + qi[r]);
+    if (DROP) rk[r] = drop_row_key(seed, ((unsigned long long)b * a.H + h) * a.seq_rows + qi[r]);
   }
   mbar_wait(bar, 0);
 
@@ -245,14 +246,13 @@ extern "C" int sv_attention_visit_all_blocks(int on) {
   return SV_OK;
 }
 
-extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
-                                             int k_rs, const void *v, long long v_bs, int v_rs, void *out, long long o_bs,
-                                             int o_rs, const unsigned char *key_padding_mask, const float *spatial_w,
-                                             int spatial_heads, const float *pairwise_locs, int B, int H, int Lq, int Lk,
-                                             float scale, float *lse, float dropout_p, unsigned long long seed,
-                                             void *stream) {
+extern "C" int sv_attention_fwd_rows_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                                          const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
+                                          const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
+                                          const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, float *lse,
+                                          float dropout_p, unsigned long long seed, int seq_rows, void *stream) {
   if (!(dropout_p >= 0.f) || dropout_p >= 1.f) return SV_ERR_INVALID_ARG;
-  if (B < 0 || H < 1 || Lq < 0 || Lk < 1 || Lk > 384) return SV_ERR_INVALID_ARG;
+  if (B < 0 || H < 1 || Lq < 0 || Lk < 1 || Lk > 384 || seq_rows < Lq) return SV_ERR_INVALID_ARG;
   if (B == 0 || Lq == 0) return SV_OK;
   if (!q || !k || !v || !out) return SV_ERR_INVALID_ARG;
   if ((q_rs % 8) || (k_rs % 8) || (v_rs % 8) || (o_rs % 8) || (q_bs % 8) || (k_bs % 8) || (v_bs % 8) || (o_bs % 8))
@@ -271,6 +271,7 @@ extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int 
   a.inv_keep = 1.0f / (1.0f - dropout_p);
   a.seed = seed; a.seed_offset = sv::g_seed_offset;
   a.all_blocks = g_visit_all_blocks;
+  a.seq_rows = seq_rows;
   CUtensorMap mq, mk, mv;
   int rc = make_map(&mq, q, B, Lq, H, q_rs, q_bs);
   if (rc) return rc;
@@ -282,4 +283,15 @@ extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int 
   if (spatial_w) return launch_fwd<true, false>(mq, mk, mv, a, st);
   if (a.t16) return launch_fwd<false, true>(mq, mk, mv, a, st);
   return launch_fwd<false, false>(mq, mk, mv, a, st);
+}
+
+extern "C" int sv_attention_fwd_dropout_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
+                                             int k_rs, const void *v, long long v_bs, int v_rs, void *out, long long o_bs,
+                                             int o_rs, const unsigned char *key_padding_mask, const float *spatial_w,
+                                             int spatial_heads, const float *pairwise_locs, int B, int H, int Lq, int Lk,
+                                             float scale, float *lse, float dropout_p, unsigned long long seed,
+                                             void *stream) {
+  return sv_attention_fwd_rows_bf16(q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, out, o_bs, o_rs, key_padding_mask,
+                                    spatial_w, spatial_heads, pairwise_locs, B, H, Lq, Lk, scale, lse, dropout_p, seed,
+                                    Lq, stream);
 }

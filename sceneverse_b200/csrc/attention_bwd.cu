@@ -22,8 +22,10 @@ struct BwdArgs {
   const float *sw, *locs, *lse;      // (B,Lq,H*6) | (B,Lq,Lk,5) | (B,H,Lq)
   int B, H, Lq, Lk;
   float scale;
-  __nv_bfloat16 *dq, *dk, *dv;       // (B,L,H*64) with row stride d_rs (elements; rows of one tensor d_rs apart, scenes L * d_rs)
+  __nv_bfloat16 *dq, *dk, *dv;       // dq (B,seq_rows,*), dk / dv (B,Lk,*): rows d_rs elements apart, scenes rows * d_rs
   int d_rs;
+  int seq_rows;                      // the queries are the first Lq of seq_rows rows: dq rows [Lq, seq_rows) are zero and
+                                     // query i of (b, h) has the dropout row key (b H + h) seq_rows + i
   float *dsw;                        // (B,Lq,H*6) or null
   float *dvec;                       // (B,H,Lq)   D, written by SIDE 0, read by SIDE 1
   uint32_t t16;
@@ -90,6 +92,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
   const int b = bh / a.H, h = bh % a.H;
   const int E = a.H * DH;
   const int nblk = (NC + 63) >> 6;
+  // dq rows [Lq, seq_rows) of this head: zeros, written by the last query tile (a packed gradient whose queries are a
+  // prefix of its rows then feeds one dgrad / wgrad GEMM over all of them)
+  if (SIDE == 0 && r0 + 64 >= a.Lq)
+    for (int i = a.Lq * 8 + tid; i < a.seq_rows * 8; i += 128)
+      reinterpret_cast<uint4 *>(a.dq + ((size_t)b * a.seq_rows + (i >> 3)) * a.d_rs + h * DH)[i & 7] = make_uint4(0, 0, 0, 0);
   uint32_t live = 0u;   // the column blocks visited (attn_common.cuh, block skipping)
   // column block blk, the i-th visited one -> ring buffer i % BWD_STAGES
   auto load_cblock = [&](int i, int blk) {
@@ -124,7 +131,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
       const size_t r = ((size_t)b * a.H + h) * a.Lq + c;
       lse2s[c] = live ? a.lse[r] * LOG2E : INFINITY;
       Dv[c] = live ? a.dvec[r] : 0.f;
-      rks[c] = DROP ? drop_row_key(attn::effective_seed(a.seed, a.seed_offset), r) : 0u;
+      rks[c] = DROP ? drop_row_key(attn::effective_seed(a.seed, a.seed_offset), ((size_t)b * a.H + h) * a.seq_rows + c) : 0u;
       if (GATED) {
         const float *wp = a.sw + ((size_t)b * a.Lq + (live ? c : 0)) * (a.H * 6) + h * 6;
 #pragma unroll
@@ -188,7 +195,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
           gw[r].load(a.sw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6);
           loc[r] = a.locs + ((size_t)b * a.Lq + ri[r]) * (size_t)a.Lk * 5;
         }
-        if (DROP) rk[r] = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), rr);
+        if (DROP) rk[r] = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), ((size_t)b * a.H + h) * a.seq_rows + ri[r]);
       }
     } else {
       klive[r] = rlive[r] && !(a.kpm != nullptr && a.kpm[(size_t)b * a.Lk + ri[r]]);
@@ -202,7 +209,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
     for (int r = 0; r < 2; ++r) {
       if (!rlive[r]) continue;
       if (SIDE == 0) {
-        store_row_zero(a.dq + ((size_t)b * a.Lq + ri[r]) * a.d_rs + h * DH, cq);
+        store_row_zero(a.dq + ((size_t)b * a.seq_rows + ri[r]) * a.d_rs + h * DH, cq);
         if (GATED && (lane & 3) == 0 && a.dsw != nullptr) {
           float *g = a.dsw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6;
 #pragma unroll
@@ -327,7 +334,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
     }
     if (!rlive[r]) continue;
     if (SIDE == 0) {
-      store_row_frag(o1, r, a.dq + ((size_t)b * a.Lq + ri[r]) * a.d_rs + h * DH, cq);
+      store_row_frag(o1, r, a.dq + ((size_t)b * a.seq_rows + ri[r]) * a.d_rs + h * DH, cq);
       if (GATED && (lane & 3) == 0 && a.dsw != nullptr) {
         float *g = a.dsw + ((size_t)b * a.Lq + ri[r]) * (a.H * 6) + h * 6;
 #pragma unroll
@@ -371,16 +378,16 @@ int launch_both(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap 
 
 }  // namespace
 
-extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
-                                             int k_rs, const void *v, long long v_bs, int v_rs, const void *o,
-                                             const void *d_o, const unsigned char *key_padding_mask,
-                                             const float *spatial_w, const float *pairwise_locs, const float *lse, int B,
-                                             int H, int Lq, int Lk, float scale, void *dq, void *dk, void *dv, int d_rs,
-                                             float *d_spatial_w, float *dvec, float dropout_p, unsigned long long seed,
-                                             void *stream) {
+extern "C" int sv_attention_bwd_rows_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                                          const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
+                                          const unsigned char *key_padding_mask, const float *spatial_w,
+                                          const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk,
+                                          float scale, void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w,
+                                          float *dvec, float dropout_p, unsigned long long seed, int seq_rows,
+                                          void *stream) {
   if (d_rs < H * attn::DH || (d_rs % 8)) return SV_ERR_INVALID_ARG;
   if (!(dropout_p >= 0.f) || dropout_p >= 1.f) return SV_ERR_INVALID_ARG;
-  if (B < 0 || H < 1 || Lq < 1 || Lk < 1 || Lq > 384 || Lk > 384) return SV_ERR_INVALID_ARG;
+  if (B < 0 || H < 1 || Lq < 1 || Lk < 1 || Lq > 384 || Lk > 384 || seq_rows < Lq) return SV_ERR_INVALID_ARG;
   if (B == 0) return SV_OK;
   if (!q || !k || !v || !o || !d_o || !lse || !dq || !dk || !dv || !dvec) return SV_ERR_INVALID_ARG;
   if ((q_rs % 8) || (k_rs % 8) || (v_rs % 8) || (q_bs % 8) || (k_bs % 8) || (v_bs % 8)) return SV_ERR_INVALID_ARG;
@@ -397,6 +404,7 @@ extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int 
   a.B = B; a.H = H; a.Lq = Lq; a.Lk = Lk; a.scale = scale;
   a.dq = (__nv_bfloat16 *)dq; a.dk = (__nv_bfloat16 *)dk; a.dv = (__nv_bfloat16 *)dv;
   a.d_rs = d_rs;
+  a.seq_rows = seq_rows;
   a.dsw = d_spatial_w; a.dvec = dvec;
   a.t16 = drop_threshold(dropout_p);
   a.inv_keep = 1.0f / (1.0f - dropout_p);
@@ -415,4 +423,16 @@ extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int 
   if (spatial_w) return launch_both<true, false>(mq, mk, mv, mo, a, st);
   if (a.t16) return launch_both<false, true>(mq, mk, mv, mo, a, st);
   return launch_both<false, false>(mq, mk, mv, mo, a, st);
+}
+
+extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,
+                                             int k_rs, const void *v, long long v_bs, int v_rs, const void *o,
+                                             const void *d_o, const unsigned char *key_padding_mask,
+                                             const float *spatial_w, const float *pairwise_locs, const float *lse, int B,
+                                             int H, int Lq, int Lk, float scale, void *dq, void *dk, void *dv, int d_rs,
+                                             float *d_spatial_w, float *dvec, float dropout_p, unsigned long long seed,
+                                             void *stream) {
+  return sv_attention_bwd_rows_bf16(q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, o, d_o, key_padding_mask, spatial_w,
+                                    pairwise_locs, lse, B, H, Lq, Lk, scale, dq, dk, dv, d_rs, d_spatial_w, dvec, dropout_p,
+                                    seed, Lq, stream);
 }

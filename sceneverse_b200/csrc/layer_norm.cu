@@ -33,6 +33,7 @@ struct LnArgs {
   float inv_keep;
   unsigned long long seed;
   const unsigned long long *seed_offset;  // device counter added to the seed at run time (or null)
+  int key_stride;                  // row r draws its dropout mask with the row key r * key_stride
 };
 
 template <typename T>
@@ -96,7 +97,7 @@ __global__ void __launch_bounds__(256) ln_fwd_kernel(const LnArgs a) {
     const size_t base8 = (size_t)row * nch;
     float v[MAXCH][8];
     uint32_t rk = 0;
-    if (DROP) rk = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), (unsigned long long)row);
+    if (DROP) rk = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), (unsigned long long)row * a.key_stride);
     float sum = 0.f;
 #pragma unroll
     for (int ch = 0; ch < MAXCH; ++ch) {
@@ -200,7 +201,7 @@ __global__ void __launch_bounds__(256, 2) ln_bwd_fused_kernel(const LnArgs a) {
     s1 = warp_sum(s1) * invD;
     s2 = warp_sum(s2) * invD;
     uint32_t rk = 0;
-    if (DROP) rk = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), (unsigned long long)row);
+    if (DROP) rk = drop_row_key(attn::effective_seed(a.seed, a.seed_offset), (unsigned long long)row * a.key_stride);
 #pragma unroll
     for (int ch = 0; ch < MAXCH; ++ch) {
       const int c = lane + 32 * ch;
@@ -399,10 +400,11 @@ bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 
 
 extern "C" int sv_layer_norm_scratch_floats(int D) { return D > 0 ? BWD_MAX_BLOCKS * 2 * D : 0; }
 
-extern "C" int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf16, int R, int D, const float *gamma,
-                                 const float *beta, float eps, float dropout_p, unsigned long long seed, void *y,
-                                 void *s, float *mean, float *rstd, void *stream) {
-  if (R < 0 || D < 8 || (D % 8) || D > 1024 || !(dropout_p >= 0.f) || dropout_p >= 1.f) return SV_ERR_INVALID_ARG;
+extern "C" int sv_layer_norm_fwd_rows(const void *x, const void *residual, int io_bf16, int R, int D, const float *gamma,
+                                      const float *beta, float eps, float dropout_p, unsigned long long seed, void *y,
+                                      void *s, float *mean, float *rstd, int row_key_stride, void *stream) {
+  if (R < 0 || D < 8 || (D % 8) || D > 1024 || !(dropout_p >= 0.f) || dropout_p >= 1.f || row_key_stride < 1)
+    return SV_ERR_INVALID_ARG;
   if (R == 0) return SV_OK;
   const bool drop = dropout_p > 0.f, has_res = residual != nullptr;
   if (!x || !gamma || !beta || !y || !mean || !rstd || ((drop || has_res) && !s)) return SV_ERR_INVALID_ARG;
@@ -412,7 +414,7 @@ extern "C" int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf1
   LnArgs a{};
   a.x = x; a.res = residual; a.y = y; a.s_out = s; a.gamma = gamma; a.beta = beta; a.mean = mean; a.rstd = rstd;
   a.R = R; a.D = D; a.eps = eps; a.t16 = attn::drop_threshold(dropout_p); a.inv_keep = 1.0f / (1.0f - dropout_p);
-  a.seed = seed; a.seed_offset = sv::g_seed_offset;
+  a.seed = seed; a.seed_offset = sv::g_seed_offset; a.key_stride = row_key_stride;
   cudaStream_t st = (cudaStream_t)stream;
   const int maxch = (D + 255) / 256;
   const bool d = a.t16 != 0;
@@ -432,10 +434,12 @@ extern "C" int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf1
   }
 }
 
-extern "C" int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma,
-                                     const float *mean, const float *rstd, float dropout_p, unsigned long long seed, void *ds,
-                                     void *dx, float *dgamma, float *dbeta, int accumulate, float *scratch, void *stream) {
-  if (R < 1 || D < 8 || (D % 8) || D > 1024 || !(dropout_p >= 0.f) || dropout_p >= 1.f) return SV_ERR_INVALID_ARG;
+extern "C" int sv_layer_norm_bwd_rows(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma,
+                                      const float *mean, const float *rstd, float dropout_p, unsigned long long seed,
+                                      void *ds, void *dx, float *dgamma, float *dbeta, int accumulate, float *scratch,
+                                      int row_key_stride, void *stream) {
+  if (R < 1 || D < 8 || (D % 8) || D > 1024 || !(dropout_p >= 0.f) || dropout_p >= 1.f || row_key_stride < 1)
+    return SV_ERR_INVALID_ARG;
   const bool drop = dropout_p > 0.f;
   if (!g || !s || !gamma || !mean || !rstd || !ds || !dgamma || !dbeta || !scratch || (drop && !dx)) return SV_ERR_INVALID_ARG;
   if (!aligned16(g) || !aligned16(s) || !aligned16(gamma) || !aligned16(ds) || (dx && !aligned16(dx))) return SV_ERR_INVALID_ARG;
@@ -443,6 +447,7 @@ extern "C" int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, 
   a.g = g; a.s_in = s; a.ds = ds; a.dx = dx; a.gamma = gamma; a.mean = const_cast<float *>(mean);
   a.rstd = const_cast<float *>(rstd); a.partials = scratch;
   a.R = R; a.D = D; a.t16 = attn::drop_threshold(dropout_p); a.inv_keep = 1.0f / (1.0f - dropout_p); a.seed = seed; a.seed_offset = sv::g_seed_offset;
+  a.key_stride = row_key_stride;
   cudaStream_t st = (cudaStream_t)stream;
   const int maxch = (D + 255) / 256;
   const bool d = a.t16 != 0;
@@ -460,6 +465,19 @@ extern "C" int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, 
     case 3: return launch_bwd<float, 3>(a, d, dgamma, dbeta, accumulate, st);
     default: return launch_bwd<float, 4>(a, d, dgamma, dbeta, accumulate, st);
   }
+}
+
+extern "C" int sv_layer_norm_fwd(const void *x, const void *residual, int io_bf16, int R, int D, const float *gamma,
+                                 const float *beta, float eps, float dropout_p, unsigned long long seed, void *y,
+                                 void *s, float *mean, float *rstd, void *stream) {
+  return sv_layer_norm_fwd_rows(x, residual, io_bf16, R, D, gamma, beta, eps, dropout_p, seed, y, s, mean, rstd, 1, stream);
+}
+
+extern "C" int sv_layer_norm_bwd_acc(const void *g, const void *s, int io_bf16, int R, int D, const float *gamma,
+                                     const float *mean, const float *rstd, float dropout_p, unsigned long long seed, void *ds,
+                                     void *dx, float *dgamma, float *dbeta, int accumulate, float *scratch, void *stream) {
+  return sv_layer_norm_bwd_rows(g, s, io_bf16, R, D, gamma, mean, rstd, dropout_p, seed, ds, dx, dgamma, dbeta, accumulate,
+                                scratch, 1, stream);
 }
 
 extern "C" int sv_l2norm_fwd(const void *x, int io_bf16, int R, int D, float eps, void *y, float *norm, void *stream) {

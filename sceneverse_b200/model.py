@@ -39,36 +39,70 @@ class BERTLanguageEncoder(nn.Module):
         self.model = BertModel(self.bert_config)  # no network: random init instead of from_pretrained(weights)
         _fuse_bert_layer_norms(self.model)
 
-    def forward(self, txt_ids, txt_masks, **kwargs):
-        return self.model(txt_ids, txt_masks).last_hidden_state
+    def forward(self, txt_ids, txt_masks, cls_only=False, **kwargs):
+        """(B, L, D) last hidden state; cls_only: only its first row (B, D), for which the last layer runs its attention
+        output projection, LayerNorms and FFN on that row alone (`_bert_cls_layer_forward`).  The values and dropout
+        masks are the same either way."""
+        last = self.model.encoder.layer[-1]
+        if not hasattr(last, "cls_only"):
+            return self.model(txt_ids, txt_masks).last_hidden_state[:, 0] if cls_only else \
+                self.model(txt_ids, txt_masks).last_hidden_state
+        last.cls_only = cls_only
+        try:
+            h = self.model(txt_ids, txt_masks).last_hidden_state
+        finally:
+            last.cls_only = False
+        return h[:, 0] if cls_only else h
 
 
-def _bert_output_forward(self, hidden_states, input_tensor):
+def _bert_output_forward(self, hidden_states, input_tensor, row_key_stride=1):
     """BertSelfOutput / BertOutput tail LayerNorm(input + dropout(dense(h))) through the fused native kernel."""
     h = ops.linear(hidden_states, self.dense.weight, self.dense.bias)
-    return self.LayerNorm(h, residual=input_tensor, dropout_p=self.dropout.p if self.training else 0.0)
+    return self.LayerNorm(h, residual=input_tensor, dropout_p=self.dropout.p if self.training else 0.0,
+                          row_key_stride=row_key_stride)
 
 
-def _bert_self_attention_forward(self, hidden_states, attention_mask=None, past_key_values=None, **kwargs):
+def _bert_self_attention_forward(self, hidden_states, attention_mask=None, past_key_values=None, query_rows=None, **kwargs):
     """BertSelfAttention through ops.attention (native wgmma forward / backward with in-kernel attention dropout on
     CUDA bf16).  `attention_mask` is the padding mask HF prepared for its SDPA path: None, or (B,1,Lq,Lk) with True /
-    0.0 = attend (identical rows), from which the (B,Lk) key-padding mask is read back."""
+    0.0 = attend (identical rows), from which the (B,Lk) key-padding mask is read back.  query_rows: only the first rows
+    attend (ops.attention_packed)."""
     qkv = ops.linear_packed(hidden_states, [self.query, self.key, self.value])   # one GEMM, [q | k | v]
     kpm = None
     if attention_mask is not None:
         row = attention_mask[:, 0, 0, :]
         kpm = row.logical_not() if row.dtype == torch.bool else row < 0
     out = ops.attention_packed(qkv, self.num_attention_heads, key_padding_mask=kpm,
-                               dropout_p=self.dropout.p if self.training else 0.0)
+                               dropout_p=self.dropout.p if self.training else 0.0, query_rows=query_rows)
     return out, None
 
 
 def _bert_feed_forward_chunk(self, attention_output):
     """BertLayer.feed_forward_chunk (BertIntermediate: dense + gelu; BertOutput: dense, dropout, LayerNorm(+ residual)) as
-    one ops.ffn (two native GEMMs, gelu in the first epilogue) + the fused dropout / residual / LayerNorm kernel."""
+    one ops.ffn (two native GEMMs, gelu in the first epilogue) + the fused dropout / residual / LayerNorm kernel.  (HF
+    counts this method's parameters, so the row-key stride lives in _bert_feed_forward.)"""
+    return _bert_feed_forward(self, attention_output)
+
+
+def _bert_feed_forward(self, attention_output, row_key_stride=1):
     inter, out = self.intermediate.dense, self.output
     h = ops.ffn(attention_output, inter.weight, inter.bias, out.dense.weight, out.dense.bias, activation="gelu")
-    return out.LayerNorm(h, residual=attention_output, dropout_p=out.dropout.p if self.training else 0.0)
+    return out.LayerNorm(h, residual=attention_output, dropout_p=out.dropout.p if self.training else 0.0,
+                         row_key_stride=row_key_stride)
+
+
+def _bert_cls_layer_forward(self, hidden_states, attention_mask=None, *args, **kwargs):
+    """BertLayer.forward of the last layer.  With `cls_only` set (BERTLanguageEncoder(..., cls_only=True)) only row 0 of
+    each sequence leaves the layer, so only that row is computed past the packed q | k | v projection, which still runs on
+    every row (its gradient stays one dgrad and one wgrad GEMM): 1-query attention over all keys, the output projection
+    with residual h[:, :1], and the FFN.  Both LayerNorms key their dropout rows by b * L, so every dropout mask, and
+    every value of row 0, is the one of the full layer."""
+    if not self.cls_only:
+        return type(self).forward(self, hidden_states, attention_mask, *args, **kwargs)
+    L = hidden_states.shape[1]
+    ctx, _ = self.attention.self(hidden_states, attention_mask, query_rows=1)
+    attention_output = self.attention.output(ctx, hidden_states[:, :1], row_key_stride=L)
+    return _bert_feed_forward(self, attention_output, row_key_stride=L)
 
 
 def _fuse_bert_layer_norms(bert):
@@ -82,10 +116,14 @@ def _fuse_bert_layer_norms(bert):
     for layer in bert.encoder.layer:
         for tail in (layer.attention.output, layer.output):
             tail.forward = types.MethodType(_bert_output_forward, tail)
-        if getattr(bert.config, "hidden_act", "gelu") == "gelu" and getattr(layer, "chunk_size_feed_forward", 0) == 0:
+        ffn = getattr(bert.config, "hidden_act", "gelu") == "gelu" and getattr(layer, "chunk_size_feed_forward", 0) == 0
+        if ffn:
             layer.feed_forward_chunk = types.MethodType(_bert_feed_forward_chunk, layer)
         if layer.attention.self.attention_head_size == 64:
             layer.attention.self.forward = types.MethodType(_bert_self_attention_forward, layer.attention.self)
+            if ffn and layer is bert.encoder.layer[-1]:
+                layer.cls_only = False
+                layer.forward = types.MethodType(_bert_cls_layer_forward, layer)
 
 
 def no_decay_param_group(parameters, lr):
@@ -122,7 +160,8 @@ class OpenVocab(nn.Module):
         if hook is not None and lang.requires_grad:
             lang.register_hook(hook)       # train.PretrainStep: launch point of the early gradient all-reduce
         if self.use_scene_cap:
-            data_dict['scene_text_embed'] = self.lang_encoder(data_dict['scene_txt_ids'], data_dict['scene_txt_masks'])[:, 0]
+            data_dict['scene_text_embed'] = self.lang_encoder(data_dict['scene_txt_ids'], data_dict['scene_txt_masks'],
+                                                              cls_only=True)
         obj, obj_pre, obj_cls_raw = self.point_encoder(data_dict['obj_fts'].float(), data_dict['obj_locs'],
                                                        data_dict['obj_masks'], data_dict['obj_sem_masks'],
                                                        data_dict.get('obj_labels'), data_dict['cur_step'],

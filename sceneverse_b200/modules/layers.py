@@ -51,10 +51,11 @@ def route_linears(module):
 
 class LayerNorm(nn.LayerNorm):
     """nn.LayerNorm (same parameters / state_dict) whose forward is the fused native dropout + residual + LayerNorm:
-    norm(x, residual=r, dropout_p=p) == LayerNorm(r + dropout(x))."""
+    norm(x, residual=r, dropout_p=p) == LayerNorm(r + dropout(x)); row_key_stride as in ops.layer_norm."""
 
-    def forward(self, x, residual=None, dropout_p=0.0):
-        return ops.layer_norm(x, self.weight, self.bias, self.eps, residual=residual, dropout_p=dropout_p)
+    def forward(self, x, residual=None, dropout_p=0.0, row_key_stride=1):
+        return ops.layer_norm(x, self.weight, self.bias, self.eps, residual=residual, dropout_p=dropout_p,
+                              row_key_stride=row_key_stride)
 
 
 def get_mlp_head(input_size, hidden_size, output_size, dropout=0):

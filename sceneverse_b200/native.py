@@ -34,10 +34,11 @@ def _mask_bytes(mask):
 
 
 def attention(q, k, v, num_heads, key_padding_mask=None, spatial_w=None, spatial_heads=0, pairwise_locs=None,
-              return_lse=False, dropout_p=0.0, seed=0):
+              return_lse=False, dropout_p=0.0, seed=0, seq_rows=None):
     """Fused attention forward: q (B,Lq,E), k/v (B,Lk,E) bf16 (views with a contiguous last dim are fine), head dim 64.
     key_padding_mask (B,Lk) bool, True = ignore.  spatial_w (B,Lq,spatial_heads*6) + pairwise_locs (B,Lq,Lk,5) switch on the
-    MultiHeadAttentionSpatial 'cond' gate.  Returns (B,Lq,E) bf16."""
+    MultiHeadAttentionSpatial 'cond' gate.  seq_rows (default Lq): the queries are the first Lq rows of a sequence of
+    seq_rows rows and draw that sequence's dropout masks.  Returns (B,Lq,E) bf16."""
     B, Lq, E = q.shape
     Lk = k.shape[1]
     assert E == num_heads * 64 and q.dtype == k.dtype == v.dtype == torch.bfloat16
@@ -49,29 +50,33 @@ def attention(q, k, v, num_heads, key_padding_mask=None, spatial_w=None, spatial
         sw = spatial_w.float().contiguous()
         locs = pairwise_locs.float().contiguous()
     lse = torch.empty((B, num_heads, Lq), dtype=torch.float32, device=q.device) if return_lse else None
-    _lib.call(_lib.gps(), "sv_attention_fwd_dropout_bf16", q.device,
+    _lib.call(_lib.gps(), "sv_attention_fwd_rows_bf16", q.device,
               q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
               v.stride(1), out.data_ptr(), out.stride(0), out.stride(1), _lib.ptr(kpm), _lib.ptr(sw), int(spatial_heads),
-              _lib.ptr(locs), B, num_heads, Lq, Lk, 0.125, _lib.ptr(lse), float(dropout_p), int(seed))
+              _lib.ptr(locs), B, num_heads, Lq, Lk, 0.125, _lib.ptr(lse), float(dropout_p), int(seed),
+              Lq if seq_rows is None else int(seq_rows))
     return (out, lse) if return_lse else out
 
 
 def attention_backward(q, k, v, out, grad_out, lse, num_heads, key_padding_mask=None, spatial_w=None, pairwise_locs=None,
-                       dropout_p=0.0, seed=0, packed_grad=None):
+                       dropout_p=0.0, seed=0, packed_grad=None, seq_rows=None):
     """Gradients of `attention` (gate requires one weight set per head).  Returns (dq, dk, dv, d_spatial_w or None).
-    packed_grad: a (B, L, 3E) bf16 buffer (self-attention on a packed QKV projection): dq / dk / dv are written straight
-    into its three column slices and returned as views."""
+    seq_rows as in `attention`: dq is then (B, seq_rows, E), its rows past Lq zero.
+    packed_grad: a (B, L, 3E) bf16 buffer (self-attention on a packed QKV projection, L = Lk = seq_rows): dq / dk / dv are
+    written straight into its three column slices and returned as views."""
     B, Lq, E = q.shape
     Lk = k.shape[1]
+    seq_rows = Lq if seq_rows is None else int(seq_rows)
     dev = q.device
     grad_out = grad_out.to(torch.bfloat16).contiguous()
     out = out.contiguous()
     if packed_grad is not None:
-        assert Lq == Lk and packed_grad.shape == (B, Lq, 3 * E) and packed_grad.is_contiguous() and packed_grad.dtype == torch.bfloat16
+        assert seq_rows == Lk and packed_grad.shape == (B, Lk, 3 * E) and packed_grad.is_contiguous() and \
+            packed_grad.dtype == torch.bfloat16
         dq, dk, dv = packed_grad[..., :E], packed_grad[..., E:2 * E], packed_grad[..., 2 * E:]
         d_rs = 3 * E
     else:
-        dq = torch.empty((B, Lq, E), dtype=torch.bfloat16, device=dev)
+        dq = torch.empty((B, seq_rows, E), dtype=torch.bfloat16, device=dev)
         dk = torch.empty((B, Lk, E), dtype=torch.bfloat16, device=dev)
         dv = torch.empty((B, Lk, E), dtype=torch.bfloat16, device=dev)
         d_rs = E
@@ -81,11 +86,11 @@ def attention_backward(q, k, v, out, grad_out, lse, num_heads, key_padding_mask=
     if spatial_w is not None:
         sw, locs = spatial_w.float().contiguous(), pairwise_locs.float().contiguous()
         dsw = torch.empty_like(sw)
-    _lib.call(_lib.gps(), "sv_attention_bwd_strided_bf16", dev,
+    _lib.call(_lib.gps(), "sv_attention_bwd_rows_bf16", dev,
               q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
               v.stride(1), out.data_ptr(), grad_out.data_ptr(), _lib.ptr(kpm), _lib.ptr(sw), _lib.ptr(locs), lse.data_ptr(),
               B, num_heads, Lq, Lk, 0.125, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), d_rs, _lib.ptr(dsw), dvec.data_ptr(),
-              float(dropout_p), int(seed))
+              float(dropout_p), int(seed), seq_rows)
     return dq, dk, dv, dsw
 
 

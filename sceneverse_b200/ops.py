@@ -59,17 +59,20 @@ class _AttentionFn(torch.autograd.Function):
 class _AttentionPackedFn(torch.autograd.Function):
     """Self-attention on a PACKED projection qkv (B,L,3E) = [q | k | v]: the kernels read the three column slices through
     strided TMA maps and the backward writes dq | dk | dv into ONE packed gradient, so the projection's backward is a
-    single dgrad + a single wgrad GEMM (no split / cat / add kernels in between)."""
+    single dgrad + a single wgrad GEMM (no split / cat / add kernels in between).  The queries are the first `query_rows`
+    rows (all L for plain self-attention); the dropout masks are those of the same rows of the L-query call, and the packed
+    gradient's dq rows past them are zero."""
 
     @staticmethod
-    def forward(ctx, qkv, sw, locs, kpm, n_head, spatial_n_head, dropout_p, seed):
+    def forward(ctx, qkv, sw, locs, kpm, n_head, spatial_n_head, dropout_p, seed, query_rows):
         from . import native
         E = qkv.shape[-1] // 3
-        q, k, v = qkv[..., :E], qkv[..., E:2 * E], qkv[..., 2 * E:]
+        q, k, v = qkv[:, :query_rows, :E], qkv[..., E:2 * E], qkv[..., 2 * E:]
         out, lse = native.attention(q, k, v, n_head, key_padding_mask=kpm, spatial_w=sw, spatial_heads=spatial_n_head,
-                                    pairwise_locs=locs, return_lse=True, dropout_p=dropout_p, seed=seed)
+                                    pairwise_locs=locs, return_lse=True, dropout_p=dropout_p, seed=seed,
+                                    seq_rows=qkv.shape[1])
         ctx.save_for_backward(qkv, out, lse, sw, locs, kpm)
-        ctx.n_head, ctx.drop = n_head, (dropout_p, seed)
+        ctx.n_head, ctx.drop, ctx.query_rows = n_head, (dropout_p, seed), query_rows
         return out
 
     @staticmethod
@@ -77,11 +80,12 @@ class _AttentionPackedFn(torch.autograd.Function):
         from . import native
         qkv, out, lse, sw, locs, kpm = ctx.saved_tensors
         E = qkv.shape[-1] // 3
-        q, k, v = qkv[..., :E], qkv[..., E:2 * E], qkv[..., 2 * E:]
+        q, k, v = qkv[:, :ctx.query_rows, :E], qkv[..., E:2 * E], qkv[..., 2 * E:]
         dqkv = torch.empty(qkv.shape, dtype=torch.bfloat16, device=qkv.device)
         _, _, _, dsw = native.attention_backward(q, k, v, out, grad_out, lse, ctx.n_head, key_padding_mask=kpm, spatial_w=sw,
-                                                 pairwise_locs=locs, dropout_p=ctx.drop[0], seed=ctx.drop[1], packed_grad=dqkv)
-        return dqkv, dsw, None, None, None, None, None, None
+                                                 pairwise_locs=locs, dropout_p=ctx.drop[0], seed=ctx.drop[1], packed_grad=dqkv,
+                                                 seq_rows=qkv.shape[1])
+        return dqkv, dsw, None, None, None, None, None, None, None
 
 
 def _packed_ok(qkv, num_heads):
@@ -90,20 +94,23 @@ def _packed_ok(qkv, num_heads):
         and qkv.is_contiguous() and qkv.shape[1] <= 384
 
 
-def attention_packed(qkv, num_heads, key_padding_mask=None, dropout_p=0.0):
-    """Self-attention on qkv (B,L,3E) = [q | k | v] -> (B,L,E)."""
+def attention_packed(qkv, num_heads, key_padding_mask=None, dropout_p=0.0, query_rows=None):
+    """Self-attention on qkv (B,L,3E) = [q | k | v] -> (B,L,E).  query_rows = n < L: only the first n rows attend (to all
+    L keys) -> (B,n,E), with the dropout masks those rows have in the full call (native path)."""
+    L = qkv.shape[1]
+    n = L if query_rows is None else int(query_rows)
     if _packed_ok(qkv, num_heads):
         return _AttentionPackedFn.apply(qkv, None, None, key_padding_mask, num_heads, 0, float(dropout_p),
-                                        _next_dropout_seed() if dropout_p > 0.0 else 0)
+                                        _next_dropout_seed() if dropout_p > 0.0 else 0, n)
     q, k, v = qkv.chunk(3, dim=-1)
-    return attention(q, k, v, num_heads, key_padding_mask=key_padding_mask, dropout_p=dropout_p)
+    return attention(q[:, :n], k, v, num_heads, key_padding_mask=key_padding_mask, dropout_p=dropout_p)
 
 
 def spatial_attention_packed(qkv, spatial_weights, pairwise_locs, n_head, spatial_n_head, key_padding_mask=None):
     """MultiHeadAttentionSpatial core on a packed projection; returns (out, None)."""
     if _packed_ok(qkv, n_head) and spatial_n_head == n_head:
         return _AttentionPackedFn.apply(qkv, spatial_weights.float(), pairwise_locs.float(), key_padding_mask, n_head,
-                                        spatial_n_head, 0.0, 0), None
+                                        spatial_n_head, 0.0, 0, qkv.shape[1]), None
     q, k, v = qkv.chunk(3, dim=-1)
     return spatial_attention(q, k, v, spatial_weights, pairwise_locs, n_head, spatial_n_head, key_padding_mask=key_padding_mask)
 
@@ -729,10 +736,11 @@ def padded_vocab_linear(h, weight, bias):
 
 class _LayerNormFn(torch.autograd.Function):
     """y = LayerNorm(residual + dropout(x)) in one native pass; the backward regenerates the dropout mask and produces
-    d(x), d(residual), d(gamma), d(beta) (gamma / beta partial sums reduced in a fixed order)."""
+    d(x), d(residual), d(gamma), d(beta) (gamma / beta partial sums reduced in a fixed order).  Row r draws the dropout
+    mask of row r * key_stride."""
 
     @staticmethod
-    def forward(ctx, x, residual, gamma, beta, eps, p, seed):
+    def forward(ctx, x, residual, gamma, beta, eps, p, seed, key_stride=1):
         from . import _lib
         D = x.shape[-1]
         x2 = x.reshape(-1, D)
@@ -742,11 +750,11 @@ class _LayerNormFn(torch.autograd.Function):
         y = torch.empty_like(x2)
         s = torch.empty_like(x2) if need_s else None
         stats = torch.empty((2, R), dtype=torch.float32, device=x.device)
-        _lib.call(_lib.gps(), "sv_layer_norm_fwd", x.device, x2.data_ptr(), _lib.ptr(r2), 1 if x.dtype == torch.bfloat16 else 0,
-                  R, D, gamma.data_ptr(), beta.data_ptr(), float(eps), float(p), int(seed), y.data_ptr(), _lib.ptr(s),
-                  stats[0].data_ptr(), stats[1].data_ptr())
+        _lib.call(_lib.gps(), "sv_layer_norm_fwd_rows", x.device, x2.data_ptr(), _lib.ptr(r2),
+                  1 if x.dtype == torch.bfloat16 else 0, R, D, gamma.data_ptr(), beta.data_ptr(), float(eps), float(p), int(seed),
+                  y.data_ptr(), _lib.ptr(s), stats[0].data_ptr(), stats[1].data_ptr(), int(key_stride))
         ctx.save_for_backward(s if need_s else x2, gamma, stats)
-        ctx.meta = (float(p), int(seed), residual is not None, x.shape)
+        ctx.meta = (float(p), int(seed), residual is not None, x.shape, int(key_stride))
         ctx.params = (gamma, beta)
         return y.view(x.shape)
 
@@ -754,7 +762,7 @@ class _LayerNormFn(torch.autograd.Function):
     def backward(ctx, g):
         from . import _lib
         s, gamma, stats = ctx.saved_tensors
-        p, seed, has_res, shape = ctx.meta
+        p, seed, has_res, shape, key_stride = ctx.meta
         R, D = s.shape
         g2 = g.reshape(R, D).to(s.dtype).contiguous()
         ds = torch.empty_like(s)
@@ -765,11 +773,12 @@ class _LayerNormFn(torch.autograd.Function):
         dg_t, db_t = (pg.grad, pb.grad) if direct else (dgb[0], dgb[1])
         lib = _lib.gps()
         scratch = torch.empty(lib.sv_layer_norm_scratch_floats(D), dtype=torch.float32, device=s.device)
-        _lib.call(lib, "sv_layer_norm_bwd_acc", s.device, g2.data_ptr(), s.data_ptr(), 1 if s.dtype == torch.bfloat16 else 0, R,
-                  D, gamma.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), p, seed, ds.data_ptr(), _lib.ptr(dx),
-                  dg_t.data_ptr(), db_t.data_ptr(), 1 if direct else 0, scratch.data_ptr())
+        _lib.call(lib, "sv_layer_norm_bwd_rows", s.device, g2.data_ptr(), s.data_ptr(), 1 if s.dtype == torch.bfloat16 else 0,
+                  R, D, gamma.data_ptr(), stats[0].data_ptr(), stats[1].data_ptr(), p, seed, ds.data_ptr(), _lib.ptr(dx),
+                  dg_t.data_ptr(), db_t.data_ptr(), 1 if direct else 0, scratch.data_ptr(), key_stride)
         d_x = (dx if dx is not None else ds).view(shape)
-        return d_x, (ds.view(shape) if has_res else None), (None if direct else dgb[0]), (None if direct else dgb[1]), None, None, None
+        return d_x, (ds.view(shape) if has_res else None), (None if direct else dgb[0]), (None if direct else dgb[1]), None, \
+            None, None, None
 
 
 def _autocast_on():
@@ -779,11 +788,12 @@ def _autocast_on():
         return torch.is_autocast_enabled()
 
 
-def layer_norm(x, weight, bias, eps=1e-5, residual=None, dropout_p=0.0):
+def layer_norm(x, weight, bias, eps=1e-5, residual=None, dropout_p=0.0, row_key_stride=1):
     """LayerNorm(residual + dropout(x)) * weight + bias over the last dimension (post-norm block tail of
     transformers.py:145-154,311-315; plain LayerNorm with residual=None, dropout_p=0).  The caller passes dropout_p = 0
     outside training.  CUDA: one native kernel, I/O in bf16 under autocast / for bf16 inputs (statistics in fp32), else
-    fp32; CPU: the torch formulation."""
+    fp32; row r of the flattened input draws the dropout mask of row r * row_key_stride (the first token of each sequence
+    of a (B, L, D) tensor: x of shape (B, 1, D), row_key_stride = L).  CPU: the torch formulation."""
     D = x.shape[-1]
     if x.is_cuda and D % 8 == 0 and 8 <= D <= 1024 and weight is not None and bias is not None and x.numel() > 0 and \
             x.dtype in (torch.bfloat16, torch.float32, torch.float16):
@@ -794,7 +804,7 @@ def layer_norm(x, weight, bias, eps=1e-5, residual=None, dropout_p=0.0):
         if residual is not None:
             r_ = residual.to(dt).expand_as(x_).contiguous()
         return _LayerNormFn.apply(x_, r_, weight.float().contiguous(), bias.float().contiguous(), eps, float(dropout_p),
-                                  _next_dropout_seed() if dropout_p > 0.0 else 0)
+                                  _next_dropout_seed() if dropout_p > 0.0 else 0, row_key_stride)
     s = x if dropout_p == 0.0 else F.dropout(x, dropout_p, True)
     if residual is not None:
         s = residual + s
