@@ -134,6 +134,25 @@ int sv_attention_bwd_rows_bf16(const void *q, long long q_bs, int q_rs, const vo
                                int d_rs, float *d_spatial_w, float *dvec, float dropout_p, unsigned long long seed,
                                int seq_rows, void *stream);
 
+/* The same forward and backward for sequences of up to 2048 queries and 2048 keys (scenes of more than 384 objects, the
+ * joint text + object sequence, captions up to BERT's 512 positions).  Parameters, results, dropout masks and the other
+ * checks are those of sv_attention_fwd_rows_bf16 / sv_attention_bwd_rows_bf16; 1 <= Lk <= 2048 and Lq <= 2048 (the
+ * backward: 1 <= Lq), anything larger is rejected.  The forward streams K and V through a two-stage TMA ring instead of
+ * keeping them resident (at most 66 KB of shared memory per CTA); every element is computed as in the resident forward,
+ * so on shapes both entries take (<= 384) the results are the same bits.  The backward is the same kernel pair as
+ * sv_attention_bwd_rows_bf16, with its per-column arrays sized for the call. */
+int sv_attention_fwd_long_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                               const void *v, long long v_bs, int v_rs, void *out, long long o_bs, int o_rs,
+                               const unsigned char *key_padding_mask, const float *spatial_w, int spatial_heads,
+                               const float *pairwise_locs, int B, int H, int Lq, int Lk, float scale, float *lse,
+                               float dropout_p, unsigned long long seed, int seq_rows, void *stream);
+int sv_attention_bwd_long_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                               const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
+                               const unsigned char *key_padding_mask, const float *spatial_w, const float *pairwise_locs,
+                               const float *lse, int B, int H, int Lq, int Lk, float scale, void *dq, void *dk, void *dv,
+                               int d_rs, float *d_spatial_w, float *dvec, float dropout_p, unsigned long long seed,
+                               int seq_rows, void *stream);
+
 /* Both attention directions skip every 64-key block whose keys are all masked (key_padding_mask or past Lk): such a block
  * only adds zero weights, so the results are the full sweep's bit for bit, up to the sign of a zero.  Tests: on = 1 makes
  * every launch sweep all blocks again, on = 0 (default) restores skipping. */

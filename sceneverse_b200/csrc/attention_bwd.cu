@@ -144,7 +144,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap mR1, const __grid_constant__
   fence_proxy_async_smem();
   __syncthreads();
   live = wlive[0] | wlive[1] | wlive[2] | wlive[3];
-  if (a.all_blocks || (SIDE == 1 && live)) live = (1u << nblk) - 1u;
+  if (a.all_blocks || (SIDE == 1 && live)) live = first_blocks(nblk);
   const int nlive = __popc(live);
   if (tid == 0 && nlive > 0) {
     mbar_expect_tx(&bars[BWD_STAGES], 2 * rows_bytes(r0, 4, Lr));
@@ -352,17 +352,21 @@ int launch_side(const CUtensorMap &r1, const CUtensorMap &r2, const CUtensorMap 
                 const BwdArgs &a, cudaStream_t st) {
   const int Lr = SIDE == 0 ? a.Lq : a.Lk, Lc = SIDE == 0 ? a.Lk : a.Lq;
   const size_t smem = bwd_smem_bytes<SIDE>((Lc + 15) & ~15, GATED);
-  constexpr size_t SMEM_MAX = bwd_smem_bytes<SIDE>(384, GATED);
+  // the kernel's dynamic shared-memory limit: the one of 384 columns until a launch needs more (the long entry), then the
+  // one of STREAM_MAX columns
+  constexpr size_t SMEM_RESIDENT = bwd_smem_bytes<SIDE>(RESIDENT_MAX, GATED);
+  constexpr size_t SMEM_LONG = bwd_smem_bytes<SIDE>(STREAM_MAX, GATED);
   auto kern = attn_bwd_kernel<SIDE, GATED, DROP>;
-  static bool configured[64] = {false};
+  static size_t configured[64] = {0};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64) return SV_ERR_INVALID_ARG;
-  if (!configured[dev]) {
-    int rc = sv::cuda_status(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX));
+  if (configured[dev] < smem) {
+    const size_t limit = smem <= SMEM_RESIDENT ? SMEM_RESIDENT : SMEM_LONG;
+    int rc = sv::cuda_status(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit));
     if (rc) return rc;
     cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-    configured[dev] = true;
+    configured[dev] = limit;
   }
   kern<<<a.B * a.H * ((Lr + 63) >> 6), 128, smem, st>>>(r1, r2, c1, c2, a);
   return sv::after_launch();
@@ -376,18 +380,15 @@ int launch_both(const CUtensorMap &mq, const CUtensorMap &mk, const CUtensorMap 
   return launch_side<1, GATED, DROP>(mk, mv, mq, mo, a, st);
 }
 
-}  // namespace
-
-extern "C" int sv_attention_bwd_rows_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
-                                          const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
-                                          const unsigned char *key_padding_mask, const float *spatial_w,
-                                          const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk,
-                                          float scale, void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w,
-                                          float *dvec, float dropout_p, unsigned long long seed, int seq_rows,
-                                          void *stream) {
+// argument checks and launches of both backward entries (Lq, Lk <= max_len)
+int attention_bwd(int max_len, const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                  const void *v, long long v_bs, int v_rs, const void *o, const void *d_o, const unsigned char *key_padding_mask,
+                  const float *spatial_w, const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk,
+                  float scale, void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w, float *dvec, float dropout_p,
+                  unsigned long long seed, int seq_rows, void *stream) {
   if (d_rs < H * attn::DH || (d_rs % 8)) return SV_ERR_INVALID_ARG;
   if (!(dropout_p >= 0.f) || dropout_p >= 1.f) return SV_ERR_INVALID_ARG;
-  if (B < 0 || H < 1 || Lq < 1 || Lk < 1 || Lq > 384 || Lk > 384 || seq_rows < Lq) return SV_ERR_INVALID_ARG;
+  if (B < 0 || H < 1 || Lq < 1 || Lk < 1 || Lq > max_len || Lk > max_len || seq_rows < Lq) return SV_ERR_INVALID_ARG;
   if (B == 0) return SV_OK;
   if (!q || !k || !v || !o || !d_o || !lse || !dq || !dk || !dv || !dvec) return SV_ERR_INVALID_ARG;
   if ((q_rs % 8) || (k_rs % 8) || (v_rs % 8) || (q_bs % 8) || (k_bs % 8) || (v_bs % 8)) return SV_ERR_INVALID_ARG;
@@ -423,6 +424,32 @@ extern "C" int sv_attention_bwd_rows_bf16(const void *q, long long q_bs, int q_r
   if (spatial_w) return launch_both<true, false>(mq, mk, mv, mo, a, st);
   if (a.t16) return launch_both<false, true>(mq, mk, mv, mo, a, st);
   return launch_both<false, false>(mq, mk, mv, mo, a, st);
+}
+
+}  // namespace
+
+extern "C" int sv_attention_bwd_rows_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                                          const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
+                                          const unsigned char *key_padding_mask, const float *spatial_w,
+                                          const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk,
+                                          float scale, void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w,
+                                          float *dvec, float dropout_p, unsigned long long seed, int seq_rows,
+                                          void *stream) {
+  return attention_bwd(RESIDENT_MAX, q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, o, d_o, key_padding_mask, spatial_w,
+                       pairwise_locs, lse, B, H, Lq, Lk, scale, dq, dk, dv, d_rs, d_spatial_w, dvec, dropout_p, seed,
+                       seq_rows, stream);
+}
+
+extern "C" int sv_attention_bwd_long_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs, int k_rs,
+                                          const void *v, long long v_bs, int v_rs, const void *o, const void *d_o,
+                                          const unsigned char *key_padding_mask, const float *spatial_w,
+                                          const float *pairwise_locs, const float *lse, int B, int H, int Lq, int Lk,
+                                          float scale, void *dq, void *dk, void *dv, int d_rs, float *d_spatial_w,
+                                          float *dvec, float dropout_p, unsigned long long seed, int seq_rows,
+                                          void *stream) {
+  return attention_bwd(STREAM_MAX, q, q_bs, q_rs, k, k_bs, k_rs, v, v_bs, v_rs, o, d_o, key_padding_mask, spatial_w,
+                       pairwise_locs, lse, B, H, Lq, Lk, scale, dq, dk, dv, d_rs, d_spatial_w, dvec, dropout_p, seed,
+                       seq_rows, stream);
 }
 
 extern "C" int sv_attention_bwd_strided_bf16(const void *q, long long q_bs, int q_rs, const void *k, long long k_bs,

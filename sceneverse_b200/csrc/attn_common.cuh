@@ -34,6 +34,8 @@ namespace attn {
 using namespace sm90;
 
 constexpr int DH = 64;
+constexpr int RESIDENT_MAX = 384;   // keys of the resident forward; Lq and Lk of the sv_attention_*_rows_bf16 entries
+constexpr int STREAM_MAX = 2048;     // Lq and Lk of the sv_attention_*_long_bf16 entries: 32 blocks of 64 = one 32-bit mask
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr float LN2 = 0.6931471805599453f;
 constexpr float LOG2_CLAMP = -19.931568569324174f;  // log2(1e-6): the reference clamps sigmoid(.) at 1e-6 before the log
@@ -90,6 +92,8 @@ struct GateW {
 };
 
 // ---- wgmma chains of one 64-row unit -----------------------------------------------------------------------------------
+// the first n column blocks (1 <= n <= 32): a mask of every block without the undefined shift by 32 at n = 32
+__device__ __forceinline__ uint32_t first_blocks(int n) { return 0xffffffffu >> (32 - n); }
 // index of the i-th set bit of `live` (the i-th visited column block), -1 past the last
 __device__ __forceinline__ int nth_block(uint32_t live, int i) {
   for (; i > 0 && live; --i) live &= live - 1u;

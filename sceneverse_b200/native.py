@@ -33,14 +33,26 @@ def _mask_bytes(mask):
     return (mask != 0).contiguous().view(torch.uint8)
 
 
+RESIDENT_MAX = 384    # Lq and Lk of sv_attention_{fwd,bwd}_rows_bf16 (include/svgps.h)
+LONG_MAX = 2048       # Lq and Lk of sv_attention_{fwd,bwd}_long_bf16
+
+
+def _long_entry(long, Lq, Lk):
+    """None: the long entry exactly when a length exceeds the resident entries' RESIDENT_MAX."""
+    return (Lq > RESIDENT_MAX or Lk > RESIDENT_MAX) if long is None else bool(long)
+
+
 def attention(q, k, v, num_heads, key_padding_mask=None, spatial_w=None, spatial_heads=0, pairwise_locs=None,
-              return_lse=False, dropout_p=0.0, seed=0, seq_rows=None):
+              return_lse=False, dropout_p=0.0, seed=0, seq_rows=None, long=None):
     """Fused attention forward: q (B,Lq,E), k/v (B,Lk,E) bf16 (views with a contiguous last dim are fine), head dim 64.
     key_padding_mask (B,Lk) bool, True = ignore.  spatial_w (B,Lq,spatial_heads*6) + pairwise_locs (B,Lq,Lk,5) switch on the
     MultiHeadAttentionSpatial 'cond' gate.  seq_rows (default Lq): the queries are the first Lq rows of a sequence of
-    seq_rows rows and draw that sequence's dropout masks.  Returns (B,Lq,E) bf16."""
+    seq_rows rows and draw that sequence's dropout masks.  long: True = sv_attention_fwd_long_bf16 (K / V streamed, Lq, Lk
+    <= 2048), False = sv_attention_fwd_rows_bf16 (K / V resident, Lk <= 384), None = the long entry only when Lq or Lk
+    exceeds 384.  Returns (B,Lq,E) bf16."""
     B, Lq, E = q.shape
     Lk = k.shape[1]
+    entry = "sv_attention_fwd_long_bf16" if _long_entry(long, Lq, Lk) else "sv_attention_fwd_rows_bf16"
     assert E == num_heads * 64 and q.dtype == k.dtype == v.dtype == torch.bfloat16
     assert q.stride(2) == 1 and k.stride(2) == 1 and v.stride(2) == 1
     out = torch.empty((B, Lq, E), dtype=torch.bfloat16, device=q.device)
@@ -50,7 +62,7 @@ def attention(q, k, v, num_heads, key_padding_mask=None, spatial_w=None, spatial
         sw = spatial_w.float().contiguous()
         locs = pairwise_locs.float().contiguous()
     lse = torch.empty((B, num_heads, Lq), dtype=torch.float32, device=q.device) if return_lse else None
-    _lib.call(_lib.gps(), "sv_attention_fwd_rows_bf16", q.device,
+    _lib.call(_lib.gps(), entry, q.device,
               q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
               v.stride(1), out.data_ptr(), out.stride(0), out.stride(1), _lib.ptr(kpm), _lib.ptr(sw), int(spatial_heads),
               _lib.ptr(locs), B, num_heads, Lq, Lk, 0.125, _lib.ptr(lse), float(dropout_p), int(seed),
@@ -59,9 +71,10 @@ def attention(q, k, v, num_heads, key_padding_mask=None, spatial_w=None, spatial
 
 
 def attention_backward(q, k, v, out, grad_out, lse, num_heads, key_padding_mask=None, spatial_w=None, pairwise_locs=None,
-                       dropout_p=0.0, seed=0, packed_grad=None, seq_rows=None):
+                       dropout_p=0.0, seed=0, packed_grad=None, seq_rows=None, long=None):
     """Gradients of `attention` (gate requires one weight set per head).  Returns (dq, dk, dv, d_spatial_w or None).
-    seq_rows as in `attention`: dq is then (B, seq_rows, E), its rows past Lq zero.
+    seq_rows as in `attention`: dq is then (B, seq_rows, E), its rows past Lq zero.  long as in `attention`:
+    sv_attention_bwd_long_bf16 (Lq, Lk <= 2048) or sv_attention_bwd_rows_bf16 (<= 384).
     packed_grad: a (B, L, 3E) bf16 buffer (self-attention on a packed QKV projection, L = Lk = seq_rows): dq / dk / dv are
     written straight into its three column slices and returned as views."""
     B, Lq, E = q.shape
@@ -86,7 +99,8 @@ def attention_backward(q, k, v, out, grad_out, lse, num_heads, key_padding_mask=
     if spatial_w is not None:
         sw, locs = spatial_w.float().contiguous(), pairwise_locs.float().contiguous()
         dsw = torch.empty_like(sw)
-    _lib.call(_lib.gps(), "sv_attention_bwd_rows_bf16", dev,
+    entry = "sv_attention_bwd_long_bf16" if _long_entry(long, Lq, Lk) else "sv_attention_bwd_rows_bf16"
+    _lib.call(_lib.gps(), entry, dev,
               q.data_ptr(), q.stride(0), q.stride(1), k.data_ptr(), k.stride(0), k.stride(1), v.data_ptr(), v.stride(0),
               v.stride(1), out.data_ptr(), grad_out.data_ptr(), _lib.ptr(kpm), _lib.ptr(sw), _lib.ptr(locs), lse.data_ptr(),
               B, num_heads, Lq, Lk, 0.125, dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), d_rs, _lib.ptr(dsw), dvec.data_ptr(),

@@ -30,6 +30,9 @@ def _next_dropout_seed():
     return (torch.initial_seed() * 0x9E3779B1 + _dropout_calls[0] * 0x85EBCA6B) & 0x7FFFFFFFFFFFFFFF
 
 
+ATTENTION_MAX_LEN = 2048   # queries and keys of the native attention (native.LONG_MAX: the long entries above 384)
+
+
 def _native_ok(*tensors):
     return all(t.is_cuda and t.dtype == torch.bfloat16 for t in tensors)
 
@@ -91,7 +94,7 @@ class _AttentionPackedFn(torch.autograd.Function):
 def _packed_ok(qkv, num_heads):
     E = qkv.shape[-1] // 3
     return qkv.is_cuda and qkv.dtype == torch.bfloat16 and qkv.dim() == 3 and qkv.shape[-1] == 3 * E and E == num_heads * 64 \
-        and qkv.is_contiguous() and qkv.shape[1] <= 384
+        and qkv.is_contiguous() and qkv.shape[1] <= ATTENTION_MAX_LEN
 
 
 def attention_packed(qkv, num_heads, key_padding_mask=None, dropout_p=0.0, query_rows=None):
@@ -489,14 +492,15 @@ def calc_pairwise_locs(obj_centers, obj_whls, eps=1e-10, pairwise_rel_type='cent
 def attention(q, k, v, num_heads, key_padding_mask=None, dropout_p=0.0):
     """Scaled-dot-product attention on packed heads: q (B,Lq,E), k/v (B,Lk,E) -> (B,Lq,E).
     key_padding_mask (B,Lk) bool, True = ignore (nn.MultiheadAttention convention).
-    bf16 CUDA tensors run on the native wgmma kernels (head dim 64, <= 384 tokens — every shape of the GPS stack) and an
-    unsupported bf16 shape RAISES: there is no silent library fallback on the product path.  fp32 tensors (CPU host-logic
-    tests, the fp32 parity path on the GPU) use the torch formulation."""
+    bf16 CUDA tensors run on the native wgmma kernels (head dim 64, <= 2048 queries and keys: K / V resident up to 384,
+    streamed above) and an unsupported bf16 shape RAISES: there is no silent library fallback on the product path.  fp32
+    tensors (CPU host-logic tests, the fp32 parity path on the GPU) use the torch formulation."""
     B, Lq, E = q.shape
     Lk, hd = k.shape[1], E // num_heads
     if _native_ok(q, k, v):
-        if hd != 64 or Lk > 384 or Lq > 384:
-            raise NotImplementedError(f"native attention supports head dim 64 and <= 384 tokens (got head dim {hd}, Lq {Lq}, Lk {Lk})")
+        if hd != 64 or Lk > ATTENTION_MAX_LEN or Lq > ATTENTION_MAX_LEN:
+            raise NotImplementedError(f"native attention supports head dim 64 and at most {ATTENTION_MAX_LEN} queries and "
+                                      f"keys (got head dim {hd}, Lq {Lq}, Lk {Lk})")
         needs_grad = torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad)
         if not needs_grad and dropout_p == 0.0:
             from . import native
@@ -519,8 +523,9 @@ def spatial_attention(q, k, v, spatial_weights, pairwise_locs, n_head, spatial_n
     native forward with a recomputed backward.  An unsupported bf16 shape raises.  fp32 tensors -> the torch formulation
     below (CPU host-logic tests, fp32 parity path)."""
     if _native_ok(q, k, v):
-        if q.shape[-1] // n_head != 64 or k.shape[1] > 384 or q.shape[1] > 384:
-            raise NotImplementedError("native spatial attention supports head dim 64 and <= 384 objects")
+        if q.shape[-1] // n_head != 64 or k.shape[1] > ATTENTION_MAX_LEN or q.shape[1] > ATTENTION_MAX_LEN:
+            raise NotImplementedError(f"native spatial attention supports head dim 64 and at most {ATTENTION_MAX_LEN} "
+                                      f"objects (got head dim {q.shape[-1] // n_head}, Lq {q.shape[1]}, Lk {k.shape[1]})")
         fn = _AttentionFn if spatial_n_head == n_head else _SpatialAttentionRecomputeFn
         out = fn.apply(q, k, v, spatial_weights.float(), pairwise_locs.float(), key_padding_mask, n_head, spatial_n_head)
         return out, None
