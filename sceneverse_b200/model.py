@@ -321,6 +321,20 @@ def pretrain_config(num_gpu=1, with_obj_between=True, text_features=None):
     }
 
 
+def pretrain_unfreeze_config(num_gpu=1, text_features=None):
+    """configs/final/all_pretrain_unfreeze.yaml (model/solver part): pretrain_config with the object encoder trainable
+    (`vision.args.freeze: False`, :214) and 100 warm-up steps (`solver.sched.args.warmup_steps`, :184).  lr 5e-4, grad_norm
+    5.0, betas (0.9, 0.98) and minimum_ratio 0.1 (:174-185) and the per-module lrs (language 1e-5, vision and grounding 1e-4,
+    :208, :226, :235) are those of all_pretrain.yaml.  PointNet++ then trains with batch-statistic BatchNorm (pn_train.py)
+    and its parameters join the vision groups of get_opt_params.  The yaml's `vision.args.path` (:215) is the ObjCls
+    checkpoint the backbone starts from: set `model.vision.args.path`, or call PretrainStep.load_pretrain, to continue
+    from one; with several GPUs the BatchNorm layers stay plain BatchNorm2d, as in the reference's OpenVocab."""
+    cfg = pretrain_config(num_gpu, text_features=text_features)
+    cfg["model"]["vision"]["args"]["freeze"] = False
+    cfg["solver"]["sched"]["args"]["warmup_steps"] = 100
+    return cfg
+
+
 def per_scene_pretrain_config(num_gpu=1, text_features=None):
     """pretrain_config as OpenVocabPerScene: the losses the reference can run per scene (lm_cls_loss, TextObjWithinBatch,
     TextObjBetweenBatch) and no scene captions.  Batches are synthetic.per_scene_batch-shaped (txt_ids (B, U, T))."""

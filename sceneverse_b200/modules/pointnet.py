@@ -200,6 +200,16 @@ class PointNetPP(nn.Module):
                 dst.copy_(src)
         self._packed = old          # _pack() left the key of the current weights
 
+    def train(self, mode=True):
+        """Leaving train mode re-derives the packed eval-mode images in place from the current weights and BatchNorm
+        running statistics.  Training changes them without a host-visible version bump (the flat AdamW of a captured step
+        writes through the flat buffer, replayed BatchNorm updates write the buffers), so neither _pack's key nor a
+        captured evaluation graph, which holds the images' addresses, would notice; EvalRunner.run and model.eval() both
+        pass through here before they read the images."""
+        if not mode and self.training and self._packed is not None:
+            self.refresh_pack_()
+        return super().train(mode)
+
     # -------------------------------------------------------------- forward
     def forward(self, features):
         """@param features: (B*N_objects, N_points, 3 + C)  ->  (B*N_objects, D)"""

@@ -265,13 +265,29 @@ def available(pc, net):
     return exchange_for(net, pc.device) is not False
 
 
-def sa_forward(sa, xyz, feat, ex=None):
+def sample_levels(net, xyz):
+    """(new_xyz, ball_idx) of each level of `net` sampled up front, or None for a level sa_forward samples itself.  A net whose
+    first two levels are sampled with 32 centres at the first (the GPS encoder) on 32..1024 points gets both levels from ONE
+    sa_sample launch (_ext.sa_sample2), whose indices are bit-exact with FPS + gather + ball query (DESIGN.md §1 a1-a3)."""
+    from .pointnet2 import _ext
+    enc = net.encoder
+    if len(enc) >= 2 and enc[0].npoint == 32 and enc[1].npoint is not None and 32 <= xyz.shape[1] <= 1024:
+        _, nx1, bi1, _, nx2, bi2 = _ext.sa_sample2(xyz, enc[0].npoint, enc[0].radius, enc[0].nsample,
+                                                   enc[1].npoint, enc[1].radius, enc[1].nsample)
+        return [(nx1, bi1), (nx2, bi2)] + [None] * (len(enc) - 2)
+    return [None] * len(enc)
+
+
+def sa_forward(sa, xyz, feat, ex=None, sampled=None):
     """One PointnetSAModule in training mode: xyz (B,N,3) f32, feat (B,N,C) point-major (f32 | bf16) -> (new_xyz, (B,np,Cout) bf16).
-    ex: the StatExchange of SyncBatchNorm layers, or None."""
-    from . import pointnet2_utils
+    ex: the StatExchange of SyncBatchNorm layers, or None.  sampled: this level's (new_xyz, ball_idx) from sample_levels, or None."""
     from .pointnet2 import _ext
     B, N, _ = xyz.shape
-    if sa.npoint is not None:
+    if sampled is not None:
+        new_xyz, bidx = sampled
+        np_, ns = sa.npoint, sa.nsample
+        X = _GroupRowsFn.apply(xyz, new_xyz, feat, bidx, np_, ns)
+    elif sa.npoint is not None:
         idx = _ext.furthest_point_sampling(xyz, sa.npoint)
         new_xyz = torch.gather(xyz, 1, idx.long()[..., None].expand(-1, -1, 3)).contiguous()
         bidx = _ext.ball_query(new_xyz, xyz, sa.radius, sa.nsample)
@@ -300,7 +316,7 @@ def forward(net, pc, exchange=None):
                            "PointNetPP.forward_generic")
     xyz = pc[..., 0:3].contiguous()
     feat = pc[..., 3:].contiguous() if pc.size(-1) > 3 else None
-    for sa in net.encoder:
-        new_xyz, feat = sa_forward(sa, xyz, feat, ex)
+    for sa, sampled in zip(net.encoder, sample_levels(net, xyz)):
+        new_xyz, feat = sa_forward(sa, xyz, feat, ex, sampled)
         xyz = new_xyz if new_xyz is not None else xyz
     return ops.linear(feat.reshape(feat.shape[0], -1), net.fc.weight, net.fc.bias)

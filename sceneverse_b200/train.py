@@ -375,11 +375,16 @@ class PretrainStep(CapturedStep):
     @torch.no_grad()
     def load_pretrain(self, path):
         """BaseTrainer.load_pretrain (trainer/build.py:174-184): every pytorch_model*.bin of `path` into the model,
-        strict=False, before the first step.  Returns (missing_keys, unexpected_keys)."""
+        strict=False, before the first step.  Returns (missing_keys, unexpected_keys).  An ObjClsStep checkpoint names its
+        backbone `point_feature_extractor.*`; that is the object encoder's PointNet++ here (the stage hand-off that
+        all_pretrain_unfreeze.yaml makes through `vision.args.path`), so those keys load into it."""
         if self.probed:
             raise RuntimeError("load_pretrain must run before the first step")
         from . import checkpoint as C
-        return self.module.model.load_state_dict(C.read_pretrain(path), strict=False)
+        sd = C.read_pretrain(path)
+        obj = "point_feature_extractor."
+        sd = {("point_encoder." + k if k.startswith(obj) else k): v for k, v in sd.items()}
+        return self.module.model.load_state_dict(sd, strict=False)
 
     def _lrs(self):
         return [g['lr'] for g in self.optimizer.param_groups]
