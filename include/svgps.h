@@ -50,7 +50,8 @@ int sv_gemm_bf16_ex(const void *A, int lda, int a_transposed, const void *B, int
                     void *stream);
 
 /* Kernel selection of the GEMM family (tests / benchmarks): 0 = heuristic (default), 1 / 2 / 4 = tiles of 64 / 128 / 192
- * output columns (128 rows each).
+ * output columns (128 rows each); + 8 / + 16 = the staged forward / dgrad on the cooperative schedule / on epilogue
+ * warpgroups (64- and 128-column tiles only; 0 = heuristic).
  * Bits 8.. are profiling switches that make the RESULT GARBAGE (timing only): 1 = the epilogue skips its body,
  * 2 = the producer skips its TMA loads. */
 int sv_gemm_force_ctas(int ctas);

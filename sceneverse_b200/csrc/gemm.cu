@@ -6,7 +6,9 @@
 //   C[M,N] = epilogue( A[M,K] x B[N,K]^T ),  bf16 operands, fp32 accumulation in registers
 //
 // Roles (384 threads): warp 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers: each issues the wgmma chain
-// for 64 rows of the 128-row tile and runs the epilogue of those rows straight from its accumulator registers.
+// for 64 rows of the 128-row tile and runs the epilogue of those rows straight from its accumulator registers.  The staged
+// forward and dgrad kernels at 64- and 128-column tiles have 640 threads instead: warpgroups 3 and 4 run the epilogues of
+// warpgroups 1 and 2, fed through shared memory, so the MMAs of the next tile overlap each tile's epilogue (see gemm_kernel).
 // Operand tiles travel global -> shared by TMA (cp.async.bulk.tensor.2d, 128-byte rows, SWIZZLE_128B) through an
 // mbarrier ring of up to 8 stages that keeps loading the next tiles while the consumers run an epilogue; either operand
 // may be stored transposed in memory ([K][rows]) and is then staged as 64-column slabs and read MN-major by wgmma —
@@ -40,7 +42,6 @@ namespace {
 using namespace sm90;
 
 constexpr int BM = 128, BK = 64;
-constexpr int NTHREADS = 384;
 constexpr int EPI_FWD = 0, EPI_DGRAD = 1, EPI_WGRAD = 2;
 
 struct GemmArgs {
@@ -108,17 +109,33 @@ constexpr int OUT_BOX = 64 * 128;
 constexpr int OUT_RING = 2 * OUT_BOX;
 constexpr int SMEM_OPTIN = 232448;   // 227 KB: the sm_90 per-block opt-in limit
 
-template <int BN, int OUT_TMA>
+template <int BN, int EPI, int OUT_TMA>
 struct GemmCfg {
+  // EW: the staged forward / dgrad epilogue runs in two warpgroups of its own (see gemm_kernel), fed the accumulators through a
+  // shared-memory hand-off of 64 x BN fp32 per MMA warpgroup.  Not at BN = 192: the hand-off (96 KB) would leave 2 stages.
+  // OUT_TMA = 2 selects it; run_gemm takes it only where a CTA gets enough tiles for the overlap to pay (pick_tile).
+  static constexpr bool EW = OUT_TMA == 2;
+  static_assert(!EW || (BN <= 128 && EPI != EPI_WGRAD), "epilogue warpgroups: staged forward / dgrad at BN <= 128 only");
+  static constexpr int THREADS = EW ? 640 : 384;
+  // Register split (setmaxnreg, NREG): the producer warpgroup gives most of its launch share to the warpgroups that hold the
+  // 64 x BN fp32 accumulators.  EW: 640 threads launch with 96 each, 128 x (24 + 2 x 96 epilogue + 2 x 128) = 60416 <= 640 x 96.
+  // The cooperative staged kernels: 384 threads launch with 168, 128 x (40 + 2 x 232) = 64512 = 384 x 168 (the 192-wide
+  // epilogue spills at a flat 168).  The per-element kernels keep one register count for all their threads.
+  static constexpr bool NREG = OUT_TMA != 0;
+  static constexpr int REG_LAUNCH = EW ? 96 : 168, REG_PRODUCER = EW ? 24 : 40, REG_EPI = 96, REG_MMA = EW ? 128 : 232;
+  static_assert(128 * (REG_PRODUCER + (EW ? 2 * REG_EPI : 0) + 2 * REG_MMA) <= THREADS * REG_LAUNCH,
+                "setmaxnreg split exceeds the launch allocation");
   static constexpr int A_STAGE = BM * BK * 2, B_STAGE = BN * BK * 2;
-  static constexpr int OUT = OUT_TMA ? 2 * OUT_RING : 0;   // the output rings of the two consumer warpgroups
-  static constexpr int BARS = 2 * 8 + 4;                   // full / empty of at most 8 stages, 2 x 2 aux-box barriers
-  // OUT_TMA: operand stages fill what is left after the output rings, 1 KB alignment slack, the 1 KB tile of ones (WGRAD
-  // bias-gradient operand) and the barriers.  The per-element kernels keep their 200 KB operand budget.
+  static constexpr int OUT = OUT_TMA ? 2 * OUT_RING : 0;   // the output rings of the two epilogue-running warpgroups
+  static constexpr int HAND = EW ? 2 * 64 * BN * 4 : 0;    // [2 MMA warpgroups][BN / 8][128 threads][4] fp32
+  static constexpr int BARS = 2 * 8 + 4 + 4;               // full / empty of at most 8 stages, 2 x 2 aux-box barriers,
+                                                           // 2 x (hand-off full, hand-off empty)
+  // OUT_TMA: operand stages fill what is left after the output rings, the hand-off, 1 KB alignment slack, the 1 KB tile of
+  // ones (WGRAD bias-gradient operand) and the barriers.  The per-element kernels keep their 200 KB operand budget.
   static constexpr int STAGES_RAW =
-      OUT_TMA ? (SMEM_OPTIN - OUT - 1024 - 1024 - BARS * 8) / (A_STAGE + B_STAGE) : (200 * 1024) / (A_STAGE + B_STAGE);
+      OUT_TMA ? (SMEM_OPTIN - OUT - HAND - 1024 - 1024 - BARS * 8) / (A_STAGE + B_STAGE) : (200 * 1024) / (A_STAGE + B_STAGE);
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + OUT + 1024 + 1024 + BARS * 8;
+  static constexpr size_t SMEM = (size_t)STAGES * (A_STAGE + B_STAGE) + OUT + HAND + 1024 + 1024 + BARS * 8;
   static_assert(SMEM <= SMEM_OPTIN, "gemm_kernel shared memory exceeds the opt-in limit");
 };
 
@@ -151,24 +168,35 @@ __device__ __forceinline__ void mma(float (&d)[BN / 2], uint64_t da, uint64_t db
   else wgmma_n192<TA, TB>(d, da, db, scale_d);
 }
 
-// OUT_TMA = 1: the epilogue stages out (and out2) in shared memory and writes them by TMA store (WGRAD: TMA reduce-add)
+// OUT_TMA = 1 or 2: the epilogue stages out (and out2) in shared memory and writes them by TMA store (WGRAD: TMA reduce-add)
 // through mapO / mapO2; 0: per-element stores (the maps are unused).  With g.aux_tma, mapO2 is the DGRAD saved activation,
 // whose boxes are loaded into the ring slots the same columns go out through.
+//
+// Schedules.  Cooperative (384 threads): warpgroups 1 and 2 each run the main loop of 64 rows of the tile, then the epilogue of
+// those rows from their accumulator registers, and only then the next tile's main loop.  Epilogue warpgroups (OUT_TMA = 2,
+// 640 threads: the staged forward / dgrad at BN <= 128): MMA warpgroup 1 + c copies its accumulator fragment into hand-off
+// buffer c ([BN / 8][128 threads][4] fp32: thread t's column group j at (j * 128 + t) * 16 bytes, conflict-free v4 accesses),
+// arrives on hand-off barrier "full" and goes straight on to the next tile's main loop; epilogue warpgroup 3 + c, thread t,
+// reads back exactly the fragment thread t of the MMA warpgroup held, runs the same epilogue body, and arrives on "empty".
+// An MMA warpgroup waits for "empty" only when an epilogue takes longer than a main loop.
 template <int BN, int EPI, int TA, int TB, int OUT_TMA>
-__global__ void __launch_bounds__(NTHREADS, 1)
+__global__ void __launch_bounds__(GemmCfg<BN, EPI, OUT_TMA>::THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
             const __grid_constant__ CUtensorMap mapO, const __grid_constant__ CUtensorMap mapO2, const GemmArgs g) {
   extern __shared__ uint8_t smem_raw[];
-  using Cfg = GemmCfg<BN, OUT_TMA>;
+  using Cfg = GemmCfg<BN, EPI, OUT_TMA>;
+  constexpr bool EW = Cfg::EW;
   constexpr int A_STAGE = Cfg::A_STAGE, B_STAGE = Cfg::B_STAGE, STAGES = Cfg::STAGES;
   uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B tiles: 1024-byte aligned
   uint8_t *sA = smem;
   uint8_t *sB = smem + STAGES * A_STAGE;
-  uint8_t *sOut = sB + STAGES * B_STAGE;                       // [2 consumer warpgroups][OUT_RING] staged output boxes
-  uint8_t *sOnes = sOut + Cfg::OUT;                            // [8][64] bf16 ones (1 KB), WGRAD bias-gradient operand
+  uint8_t *sOut = sB + STAGES * B_STAGE;                       // [2 epilogue-running warpgroups][OUT_RING] staged output boxes
+  float4 *sHand = reinterpret_cast<float4 *>(sOut + Cfg::OUT); // EW: [2][BN / 8][128] accumulator hand-off
+  uint8_t *sOnes = sOut + Cfg::OUT + Cfg::HAND;                // [8][64] bf16 ones (1 KB), WGRAD bias-gradient operand
   uint64_t *full = reinterpret_cast<uint64_t *>(sOnes + 1024);
   uint64_t *empty = full + STAGES;
-  uint64_t *auxb = empty + STAGES;                             // [2 consumer warpgroups][2 ring slots]: aux box landed
+  uint64_t *auxb = empty + STAGES;                             // [2 epilogue-running warpgroups][2 ring slots]: aux box landed
+  uint64_t *hfull = auxb + 4, *hempty = hfull + 2;             // EW: [2] hand-off written / read
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
@@ -181,19 +209,24 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full + s, 1);
-      mbar_init(empty + s, 2);   // one arrival per consumer warpgroup
+      mbar_init(empty + s, 2);   // one arrival per MMA warpgroup
     }
     for (int i = 0; i < 4; ++i) mbar_init(auxb + i, 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(hfull + i, 128);
+      mbar_init(hempty + i, 128);
+    }
     mbar_fence_init();
   }
   if (EPI == EPI_WGRAD) {
-    for (int i = threadIdx.x; i < 256; i += NTHREADS) reinterpret_cast<uint32_t *>(sOnes)[i] = 0x3F803F80u;  // bf16 1.0 pairs
+    for (int i = threadIdx.x; i < 256; i += Cfg::THREADS) reinterpret_cast<uint32_t *>(sOnes)[i] = 0x3F803F80u;  // bf16 1.0 pairs
     fence_proxy_async_smem();
   }
   __syncthreads();
 
   if (wg == 0) {
     // ------------------------------- TMA producer -------------------------------
+    if constexpr (Cfg::NREG) setmaxnreg_dec<Cfg::REG_PRODUCER>();
     if (warp == 0 && lane == 0) {
       uint32_t s = 0, ph = 1;   // waiting on parity 1 of a fresh barrier returns at once: the first pass finds every slot free
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -229,15 +262,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     return;
   }
 
-  // ------------------------------- consumers: wgmma main loop + epilogue of 64 rows -------------------------------
-  const int c = wg - 1;                 // rows [64 c, 64 c + 64) of the tile
+  // ---------------- MMA warpgroups (wgmma main loop of 64 rows) and the warpgroups that run the epilogue of those rows ----------------
+  const bool epi_wg = EW && wg >= 3;    // an epilogue warpgroup (EW); otherwise an MMA warpgroup, which in the cooperative
+                                        // schedule runs its own epilogue
+  const int c = epi_wg ? wg - 3 : wg - 1;   // rows [64 c, 64 c + 64) of the tile
   const int t = threadIdx.x & 127, w = t >> 5;
   const int r_lo = c * 64 + w * 16 + (lane >> 2);   // this thread's first accumulator row in the tile (second: + 8)
   const int cq = 2 * (lane & 3);                    // its first column inside every 8-column group
-  // A: 64 rows further into a K-major tile is 8 groups of 1024 B; in MN-major slabs it is the next slab (BK * 128 B)
-  const uint32_t a_off = (uint32_t)c * 8192u;
-  const uint32_t a_lbo = TA ? BK * 128 : 16, b_lbo = TB ? BK * 128 : 16;
-  const uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
   const unsigned long long seed = (EPI != EPI_WGRAD && g.t16) ? attn::effective_seed(g.seed, g.seed_offset) : 0ull;
   // staged output: a box holds box_j 8-column groups.  Without out2, box k of this warpgroup goes to ring slot k % 2; with
   // out2, every box step fills both slots (slot 0 the pre-activation, slot 1 the output).
@@ -254,59 +285,30 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
   // this lane's byte offsets inside a box: stmatrix / ldmatrix row addresses (bf16), or its two fp32 columns of row r_lo - 64 c
   const uint32_t sm_row = (uint32_t)(w * 16 + (lane & 7) + ((lane >> 3) & 1) * 8) * 128u, sm_x = lane & 7, sm_j = lane >> 4;
   const uint32_t f_row = (uint32_t)(w * 16 + (lane >> 2)) * 128u, f_hi = (lane >> 1) & 1, f_x = lane >> 2, f_lo = (lane & 1) * 8u;
+  float4 *hand = sHand + (size_t)c * (BN / 8) * 128;   // EW: this warpgroup pair's hand-off buffer
   uint32_t nbox = 0;
-  uint32_t s = 0, ph = 0;
-  long long p_full = 0, p_t0 = g.prof ? clock64() : 0, nks = 0;
+  uint32_t s = 0, ph = 0, hph = 0;
+  long long p_full = 0, p_t0 = g.prof ? clock64() : 0, nks = 0, p_hand = 0;
   unsigned long long p_ns0 = 0;
   if (g.prof) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(p_ns0));
-  float acc[BN / 2];
-  float accb[4];
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-    const int tt = item % n_tiles, sp = item / n_tiles;
-    const int tmi = g.n_fast ? tt / tiles_n : tt % tiles_m, tni = g.n_fast ? tt % tiles_n : tt / tiles_m;
-    const int m0 = tmi * BM, n0 = tni * BN;
-    const int ks0 = sp * kps, ks1 = min(k_steps, ks0 + kps);
-    const bool bias_tile = with_bias_grad && n0 == 0;
-    if (aux_tma && m0 + 64 * c < g.M) {
-      // the aux boxes land during the main loop; the ring is free once every thread has read the last tile's boxes (the
-      // per-element tail) and the last stores have read them
-      wg_sync(1 + c);
-      if (t == 0) {
-        bulk_wait_read<0>();
-        for (int b = 0; b < BN / 64 && n0 + 64 * b < g.N; ++b) {
-          const uint32_t slot = (nbox + (uint32_t)b) & 1u;
-          mbar_expect_tx(my_auxb + slot, OUT_BOX);
-          tma_load_2d(ring + slot * OUT_BOX, &mapO2, n0 + 64 * b, m0 + 64 * c, my_auxb + slot);
-        }
-      }
-    }
-    uint32_t prev = 0;
-    for (int ks = ks0; ks < ks1; ++ks, ++nks) {
-      long long c0 = g.prof ? clock64() : 0;
-      mbar_wait(full + s, ph);
-      if (g.prof) p_full += clock64() - c0;
-      const uint32_t a0 = smem_u32(sA + s * A_STAGE) + a_off, b0 = smem_u32(sB + s * B_STAGE);
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < BK / 16; ++kk) {
-        const uint64_t da = desc_sw128(a0 + kk * a_step, a_lbo);
-        const uint32_t sc = (ks > ks0 || kk > 0) ? 1u : 0u;
-        mma<BN, TA, TB>(acc, da, desc_sw128(b0 + kk * b_step, b_lbo), sc);
-        if (EPI == EPI_WGRAD) wgmma_n8<TA, 0>(accb, da, desc_sw128(smem_u32(sOnes) + kk * 32, 16), sc);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();      // the previous k-step's MMAs have read their slot: hand it back to the producer
-      if (ks > ks0 && t == 0) mbar_arrive(empty + prev);
-      prev = s;
-      if (++s == STAGES) { s = 0; ph ^= 1u; }
-    }
-    wgmma_wait<0>();
-    fence_regs(acc);
-    if (EPI == EPI_WGRAD) fence_regs(accb);
-    if (t == 0) mbar_arrive(empty + prev);
-    if ((g.dbg & 1) || m0 + 64 * c >= g.M) continue;   // no rows of this warpgroup to write
 
-    // ---- epilogue: element (row r_lo + 8 h, column 8 j + cq + e) is acc[4 j + 2 h + e] ----
+  // the aux boxes of the tile at (m0, n0) land while its main loop runs; the ring is free once every thread has read the last
+  // tile's boxes (the per-element tail) and the last stores have read them
+  auto load_aux = [&](int m0, int n0) {
+    wg_sync(1 + c);
+    if (t == 0) {
+      bulk_wait_read<0>();
+      for (int b = 0; b < BN / 64 && n0 + 64 * b < g.N; ++b) {
+        const uint32_t slot = (nbox + (uint32_t)b) & 1u;
+        mbar_expect_tx(my_auxb + slot, OUT_BOX);
+        tma_load_2d(ring + slot * OUT_BOX, &mapO2, n0 + 64 * b, m0 + 64 * c, my_auxb + slot);
+      }
+    }
+  };
+
+  // ---- epilogue of this thread's elements of the tile at (m0, n0): element (row r_lo + 8 h, column 8 j + cq + e) is
+  // q[2 h + e] after fetch(j, q) ----
+  auto epilogue = [&](int m0, int n0, auto &&fetch) {
     uint32_t rk[2] = {0u, 0u};
     if (EPI != EPI_WGRAD && g.t16) {
       rk[0] = attn::drop_row_key(seed, (unsigned long long)(m0 + r_lo));
@@ -375,6 +377,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
           }
         }
       }
+      float v[JB][4];   // the accumulators of column groups jc .. jc + JB - 1, then the values staged
+#pragma unroll
+      for (int jj = 0; jj < JB; ++jj) fetch(jc + jj, v[jj]);
 #pragma unroll
       for (int jj = 0; jj < JB; ++jj) {
         const int j = jc + jj;
@@ -384,7 +389,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int row = m0 + r_lo + 8 * h;
-          float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          float v0 = v[jj][2 * h], v1 = v[jj][2 * h + 1];
           if (EPI == EPI_FWD) {
             if (g.bias != nullptr) {
               v0 += bv[2 * jj];
@@ -432,8 +437,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
             }
           }
           if (tma_out) {   // staged below
-            acc[4 * j + 2 * h] = v0;
-            acc[4 * j + 2 * h + 1] = v1;
+            v[jj][2 * h] = v0;
+            v[jj][2 * h + 1] = v1;
             continue;
           }
           if (!c_ok || row >= g.M) continue;
@@ -492,8 +497,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               const uint32_t a = box + f_row + h * 1024u + ((((uint32_t)(2 * (j & 3)) + f_hi) ^ f_x) << 4) + f_lo;
-              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(acc[4 * j + 2 * h]), "f"(acc[4 * j + 2 * h + 1])
-                           : "memory");
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v[jj][2 * h]), "f"(v[jj][2 * h + 1]) : "memory");
             }
           }
         } else {
@@ -502,8 +506,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
           for (int jj = 0; jj < JB; jj += 2) {
             const int j = jc + jj;
             const uint32_t a = sm_row + (((((uint32_t)j + sm_j) & 7u) ^ sm_x) << 4);
-            stmatrix_x4(box + a, pack_bf16(acc[4 * j], acc[4 * j + 1]), pack_bf16(acc[4 * j + 2], acc[4 * j + 3]),
-                        pack_bf16(acc[4 * j + 4], acc[4 * j + 5]), pack_bf16(acc[4 * j + 6], acc[4 * j + 7]));
+            stmatrix_x4(box + a, pack_bf16(v[jj][0], v[jj][1]), pack_bf16(v[jj][2], v[jj][3]),
+                        pack_bf16(v[jj + 1][0], v[jj + 1][1]), pack_bf16(v[jj + 1][2], v[jj + 1][3]));
             if (EPI == EPI_FWD && g.out2 != nullptr)
               stmatrix_x4(ring + a, pre[2 * jj], pre[2 * jj + 1], pre[2 * jj + 2], pre[2 * jj + 3]);
           }
@@ -533,20 +537,105 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
       const uint32_t last = ring + (g.out2 != nullptr ? (uint32_t)OUT_BOX : ((nbox - 1) & 1u) * OUT_BOX);
       store_tail(sOut + (last - smem_u32(sOut)), sOut + (ring - smem_u32(sOut)), g, EPI == EPI_WGRAD, f32_out, cn, m0 + 64 * c, t);
     }
+  };
+
+  if (epi_wg) {
+    // ------------------------------- epilogue warpgroup c (EW) -------------------------------
+    if constexpr (EW) {
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const int tt = item % n_tiles;
+        const int tmi = g.n_fast ? tt / tiles_n : tt % tiles_m, tni = g.n_fast ? tt % tiles_n : tt / tiles_m;
+        const int m0 = tmi * BM, n0 = tni * BN;
+        if (m0 + 64 * c >= g.M) continue;   // no rows of this warpgroup: the MMA warpgroup hands nothing over
+        if (aux_tma) load_aux(m0, n0);
+        mbar_wait(hfull + c, hph);
+        hph ^= 1u;
+        const long long c0 = g.prof ? clock64() : 0;
+        if (!(g.dbg & 1))
+          epilogue(m0, n0, [&](int j, float (&q)[4]) {
+            const float4 x = hand[j * 128 + t];
+            q[0] = x.x; q[1] = x.y; q[2] = x.z; q[3] = x.w;
+          });
+        mbar_arrive(hempty + c);   // every read of the hand-off lies before this release
+        if (g.prof) p_hand += clock64() - c0;
+      }
+      if (t == 0) bulk_wait_all();   // the staged boxes must stay readable until the last store has read them
+      if (g.prof && t == 0 && c == 0) g.prof[(size_t)blockIdx.x * 16 + 10] = p_hand;
+    }
+    return;
+  }
+
+  if constexpr (Cfg::NREG) setmaxnreg_inc<Cfg::REG_MMA>();
+  // A: 64 rows further into a K-major tile is 8 groups of 1024 B; in MN-major slabs it is the next slab (BK * 128 B)
+  const uint32_t a_off = (uint32_t)c * 8192u;
+  const uint32_t a_lbo = TA ? BK * 128 : 16, b_lbo = TB ? BK * 128 : 16;
+  const uint32_t a_step = TA ? 2048u : 32u, b_step = TB ? 2048u : 32u;
+  float acc[BN / 2];
+  float accb[4];
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int tt = item % n_tiles, sp = item / n_tiles;
+    const int tmi = g.n_fast ? tt / tiles_n : tt % tiles_m, tni = g.n_fast ? tt % tiles_n : tt / tiles_m;
+    const int m0 = tmi * BM, n0 = tni * BN;
+    const int ks0 = sp * kps, ks1 = min(k_steps, ks0 + kps);
+    const bool bias_tile = with_bias_grad && n0 == 0;
+    if (!EW && aux_tma && m0 + 64 * c < g.M) load_aux(m0, n0);
+    uint32_t prev = 0;
+    for (int ks = ks0; ks < ks1; ++ks, ++nks) {
+      long long c0 = g.prof ? clock64() : 0;
+      mbar_wait(full + s, ph);
+      if (g.prof) p_full += clock64() - c0;
+      const uint32_t a0 = smem_u32(sA + s * A_STAGE) + a_off, b0 = smem_u32(sB + s * B_STAGE);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 16; ++kk) {
+        const uint64_t da = desc_sw128(a0 + kk * a_step, a_lbo);
+        const uint32_t sc = (ks > ks0 || kk > 0) ? 1u : 0u;
+        mma<BN, TA, TB>(acc, da, desc_sw128(b0 + kk * b_step, b_lbo), sc);
+        if (EPI == EPI_WGRAD) wgmma_n8<TA, 0>(accb, da, desc_sw128(smem_u32(sOnes) + kk * 32, 16), sc);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();      // the previous k-step's MMAs have read their slot: hand it back to the producer
+      if (ks > ks0 && t == 0) mbar_arrive(empty + prev);
+      prev = s;
+      if (++s == STAGES) { s = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (EPI == EPI_WGRAD) fence_regs(accb);
+    if (t == 0) mbar_arrive(empty + prev);
+    if (m0 + 64 * c >= g.M) continue;   // no rows of this warpgroup to write
+    if constexpr (EW) {
+      // hand the fragment to epilogue warpgroup c once it has read the previous one (a fresh barrier passes parity 1 at once)
+      const long long c0 = g.prof ? clock64() : 0;
+      mbar_wait(hempty + c, hph ^ 1u);
+      if (g.prof) p_hand += clock64() - c0;
+      hph ^= 1u;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) hand[j * 128 + t] = make_float4(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]);
+      mbar_arrive(hfull + c);
+      continue;
+    }
+    if (g.dbg & 1) continue;
+    epilogue(m0, n0, [&](int j, float (&q)[4]) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) q[i] = acc[4 * j + i];
+    });
     if (EPI == EPI_WGRAD && bias_tile && (lane & 3) == 0) {
       // every column of the N = 8 ones-product equals sum_k A[row][k]: the bias gradient of output feature `row`
       if (m0 + r_lo < g.M) atomicAdd(g.bias_grad + m0 + r_lo, accb[0]);
       if (m0 + r_lo + 8 < g.M) atomicAdd(g.bias_grad + m0 + r_lo + 8, accb[2]);
     }
   }
-  if (tma_out && t == 0) bulk_wait_all();   // the staged boxes must stay readable until the last store has read them
-  if (g.prof && t == 0 && c == 0) {   // issue-loop cycles, of which waiting for operands, k-steps, start, end, ns, epilogue
+  if (!EW && tma_out && t == 0) bulk_wait_all();   // the staged boxes must stay readable until the last store has read them
+  if (g.prof && t == 0 && c == 0) {
+    // issue-loop cycles, of which waiting for operands, k-steps, start, end, ns, epilogue (0 per element, 1 staged), schedule
+    // (0 cooperative, 1 epilogue warpgroups), cycles waiting for an empty hand-off; slot 10: the epilogue warpgroup's busy cycles
     long long *pp = g.prof + (size_t)blockIdx.x * 16;
     const long long t1 = clock64();
     unsigned long long ns1;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns1));
     pp[0] = t1 - p_t0; pp[1] = p_full; pp[2] = 0; pp[3] = nks; pp[4] = p_t0; pp[5] = t1; pp[6] = (long long)(ns1 - p_ns0);
-    pp[7] = OUT_TMA;
+    pp[7] = OUT_TMA != 0; pp[8] = EW; pp[9] = p_hand;
   }
 }
 
@@ -614,7 +703,8 @@ int device_sms(int *dev_out) {
 template <int BN, int EPI, int TA, int TB, int OUT_TMA>
 int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mo, const CUtensorMap &mo2, const GemmArgs &g,
                 cudaStream_t st) {
-  constexpr size_t smem = GemmCfg<BN, OUT_TMA>::SMEM;
+  using Cfg = GemmCfg<BN, EPI, OUT_TMA>;
+  constexpr size_t smem = Cfg::SMEM;
   auto kern = gemm_kernel<BN, EPI, TA, TB, OUT_TMA>;
   static bool configured[64] = {false};
   int dev = 0;
@@ -627,40 +717,65 @@ int launch_gemm(const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap 
   }
   const int units = ((g.M + BM - 1) / BM) * ((g.N + BN - 1) / BN) * g.splits;
   const int grid = units < sms ? units : sms;
-  kern<<<grid, NTHREADS, smem, st>>>(ma, mb, mo, mo2, g);
+  kern<<<grid, Cfg::THREADS, smem, st>>>(ma, mb, mo, mo2, g);
   return sv::after_launch();
 }
 
 // Tile selection: the persistent grid runs ceil(tiles / SMs) waves of 128 x BN tiles, and one tile costs BN times a relative
-// cost per output column measured for each width and direction (scripts/time_gemm_shapes.py at every forced width on the GPS
-// step's shapes, one H100 80GB HBM3 at 700 W, DESIGN.md §4.1), relative to the 192-wide tile.  The 64-wide tiles re-load the
-// 128-row A panel for every 64 columns; the weight gradient's 128-wide tiles leave less of their reduce-add epilogue exposed.
-float tile_cost(int epi, int bn) {
+// cost per output column measured for each width, direction and schedule (scripts/time_gemm_shapes.py at every forced width on
+// the GPS step's shapes, one H100 80GB HBM3 at 700 W, DESIGN.md §4.1), relative to the cooperative 192-wide tile.  The 64-wide
+// tiles re-load the 128-row A panel for every 64 columns; the weight gradient's 128-wide tiles leave less of their reduce-add
+// epilogue exposed.  A staged forward or dgrad at 64 or 128 columns may run its epilogue in warpgroups of its own (ew) under the
+// next tile's MMAs.  That hides every epilogue but a CTA's last, at the price of a shorter operand ring (the hand-off takes 32
+// / 64 KB), so it is offered only where a CTA gets at least three tiles, and at K > 1024 (where an epilogue is a small share
+// of a tile) only at 128 columns with at least six: elsewhere the cooperative kernel measured faster (the spatial-80, joint-130
+// and BERT-50 ffn2 forwards and the joint-130 qkv / ffn1 dgrads, K = 2048-3072; the spatial-80 ffn1 dgrad with two tiles per
+// CTA).
+struct TilePick {
+  int bn;
+  bool ew;
+};
+
+float tile_cost(int epi, int bn, bool ew) {
   static const float rel[3][3] = {{1.18f, 1.02f, 1.0f}, {1.02f, 1.0f, 1.0f}, {1.52f, 0.76f, 1.0f}};   // [epi][64, 128, 192]
-  return rel[epi][bn / 64 - 1] * (float)bn;
+  static const float rel_ew[2][2] = {{0.85f, 0.75f}, {0.99f, 0.97f}};                                 // [fwd, dgrad][64, 128]
+  return (ew ? rel_ew[epi][bn / 64 - 1] : rel[epi][bn / 64 - 1]) * (float)bn;
 }
 
-int pick_tile(int M, int N, int sms, int epi) {
+TilePick pick_tile(int M, int N, int K, int sms, int epi, bool staged, int force_bn, int force_sched) {
+  const int ew_min_waves = K <= 1024 ? 3 : 6;
   const int cand[3] = {192, 128, 64};
   float best_cost = 1e30f;
-  int best = 64;
+  TilePick best{64, false};
   const int tm = (M + BM - 1) / BM;
   for (int i = 0; i < 3; ++i) {
     const int bn = cand[i];
-    if (bn > 64 && bn - 64 >= ((N + 63) / 64) * 64) continue;          // wider than the problem by a whole 64-column slab
-    const int tiles = tm * ((N + bn - 1) / bn);
-    const float cost = (float)((tiles + sms - 1) / sms) * tile_cost(epi, bn);
-    if (cost < best_cost * 0.999f) {
-      best_cost = cost;
-      best = bn;
+    if (force_bn ? bn != force_bn : (bn > 64 && bn - 64 >= ((N + 63) / 64) * 64)) continue;   // wider than the problem
+    const int tiles = tm * ((N + bn - 1) / bn), waves = (tiles + sms - 1) / sms;
+    for (int ew = 1; ew >= 0; --ew) {
+      if (ew && !(staged && epi != EPI_WGRAD && bn <= 128)) continue;
+      if (force_sched ? (force_sched == 2) != (ew == 1) : (ew && (waves < ew_min_waves || (K > 1024 && bn == 64)))) continue;
+      const float cost = (float)waves * tile_cost(epi, bn, ew != 0);
+      if (cost < best_cost * 0.999f) {
+        best_cost = cost;
+        best = {bn, ew != 0};
+      }
     }
   }
+  if (best_cost == 1e30f) best = {force_bn ? force_bn : 64, false};   // a forced schedule the width cannot run
   return best;
 }
 
 template <int EPI, int TA, int TB>
-int dispatch(int bn, bool tma, const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mo, const CUtensorMap &mo2,
+int dispatch(TilePick tp, bool tma, const CUtensorMap &ma, const CUtensorMap &mb, const CUtensorMap &mo, const CUtensorMap &mo2,
              const GemmArgs &g, cudaStream_t st) {
+  const int bn = tp.bn;
+  if constexpr (EPI != EPI_WGRAD) {
+    if (tma && tp.ew) {
+      if (bn == 128) return launch_gemm<128, EPI, TA, TB, 2>(ma, mb, mo, mo2, g, st);
+      if (bn == 64) return launch_gemm<64, EPI, TA, TB, 2>(ma, mb, mo, mo2, g, st);
+    }
+  }
   if (tma) {
     if (bn == 192) return launch_gemm<192, EPI, TA, TB, 1>(ma, mb, mo, mo2, g, st);
     if (bn == 128) return launch_gemm<128, EPI, TA, TB, 1>(ma, mb, mo, mo2, g, st);
@@ -672,6 +787,7 @@ int dispatch(int bn, bool tma, const CUtensorMap &ma, const CUtensorMap &mb, con
 }
 
 int g_force_bn = 0;     // tests / benchmarks: 1, 2 or 4 forces 64-, 128- or 192-column tiles, 0 = heuristic
+int g_force_sched = 0;  // tests / benchmarks: staged forward / dgrad schedule, 1 cooperative, 2 epilogue warpgroups, 0 = heuristic
 int g_gemm_dbg = 0;     // profiling only (bits 8.. of sv_gemm_force_ctas): results are garbage when set
 long long *g_gemm_prof = nullptr;
 
@@ -691,7 +807,19 @@ int run_gemm(int epi, const void *A, int lda, int a_t, const void *B, int ldb, i
   g.n_fast = (long long)N <= (long long)M ? 1 : 0;
   g.dbg = g_gemm_dbg;
   g.prof = g_gemm_prof;
-  int bn = g_force_bn == 1 ? 64 : g_force_bn == 2 ? 128 : g_force_bn == 4 ? 192 : pick_tile(M, N, sms, epi);
+  // The epilogue goes out through shared memory by TMA whenever the output rows can take 16-byte-aligned boxes.  The output
+  // maps span only the columns that fill whole 16-byte units (n_tma); the last few columns of a width like 607 or 30522 are
+  // stored per element by the epilogue itself.  A TMA store clips a box at the map's inner dim only to 16-byte granularity
+  // (on H100, N = 607 in bf16 wrote column 607), so a map of width N would write into the pad columns.  The SA3 row max, the
+  // residual add and odd pitches keep the per-element stores.
+  const int esz = epi == EPI_WGRAD || g.out_f32 ? 4 : 2;
+  g.n_tma = (int)(((size_t)N * esz / 16) * 16 / esz);
+  auto al16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  const bool tma = g.rowmax == 0 && g.residual == nullptr && g.ldo >= N && ((size_t)g.ldo * esz) % 16 == 0 && g.n_tma > 0 &&
+                   al16(g.out) && (g.out2 == nullptr || (esz == 2 && al16(g.out2)));
+  const TilePick tp = pick_tile(M, N, K, sms, epi, tma, g_force_bn == 1 ? 64 : g_force_bn == 2 ? 128 : g_force_bn == 4 ? 192 : 0,
+                                g_force_sched);
+  const int bn = tp.bn;
   g.splits = 1;
   if (epi == EPI_WGRAD && g.red_out) {
     // split-K: the output of a weight gradient is small (a few dozen tiles), the contraction runs over every token
@@ -713,16 +841,6 @@ int run_gemm(int epi, const void *A, int lda, int a_t, const void *B, int ldb, i
   if (rc) return rc;
   rc = b_t ? make_map_mn(&mb, B, N, K, ldb) : make_map(&mb, B, N, K, ldb, bn);
   if (rc) return rc;
-  // The epilogue goes out through shared memory by TMA whenever the output rows can take 16-byte-aligned boxes.  The output
-  // maps span only the columns that fill whole 16-byte units (n_tma); the last few columns of a width like 607 or 30522 are
-  // stored per element by the epilogue itself.  A TMA store clips a box at the map's inner dim only to 16-byte granularity
-  // (on H100, N = 607 in bf16 wrote column 607), so a map of width N would write into the pad columns.  The SA3 row max, the
-  // residual add and odd pitches keep the per-element stores.
-  const int esz = epi == EPI_WGRAD || g.out_f32 ? 4 : 2;
-  g.n_tma = (int)(((size_t)N * esz / 16) * 16 / esz);
-  auto al16 = [](const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-  const bool tma = g.rowmax == 0 && g.residual == nullptr && g.ldo >= N && ((size_t)g.ldo * esz) % 16 == 0 && g.n_tma > 0 &&
-                   al16(g.out) && (g.out2 == nullptr || (esz == 2 && al16(g.out2)));
   CUtensorMap mo{}, mo2{};
   if (tma) {
     rc = make_out_map(&mo, g.out, M, g.n_tma, g.ldo, esz == 4);
@@ -742,11 +860,11 @@ int run_gemm(int epi, const void *A, int lda, int a_t, const void *B, int ldb, i
   }
   if (epi == EPI_FWD) {
     if (a_t)
-      return b_t ? dispatch<EPI_FWD, 1, 1>(bn, tma, ma, mb, mo, mo2, g, st) : dispatch<EPI_FWD, 1, 0>(bn, tma, ma, mb, mo, mo2, g, st);
-    return b_t ? dispatch<EPI_FWD, 0, 1>(bn, tma, ma, mb, mo, mo2, g, st) : dispatch<EPI_FWD, 0, 0>(bn, tma, ma, mb, mo, mo2, g, st);
+      return b_t ? dispatch<EPI_FWD, 1, 1>(tp, tma, ma, mb, mo, mo2, g, st) : dispatch<EPI_FWD, 1, 0>(tp, tma, ma, mb, mo, mo2, g, st);
+    return b_t ? dispatch<EPI_FWD, 0, 1>(tp, tma, ma, mb, mo, mo2, g, st) : dispatch<EPI_FWD, 0, 0>(tp, tma, ma, mb, mo, mo2, g, st);
   }
-  if (epi == EPI_DGRAD && !a_t && b_t) return dispatch<EPI_DGRAD, 0, 1>(bn, tma, ma, mb, mo, mo2, g, st);
-  if (epi == EPI_WGRAD && a_t && b_t) return dispatch<EPI_WGRAD, 1, 1>(bn, tma, ma, mb, mo, mo2, g, st);
+  if (epi == EPI_DGRAD && !a_t && b_t) return dispatch<EPI_DGRAD, 0, 1>(tp, tma, ma, mb, mo, mo2, g, st);
+  if (epi == EPI_WGRAD && a_t && b_t) return dispatch<EPI_WGRAD, 1, 1>(tp, tma, ma, mb, mo, mo2, g, st);
   return SV_ERR_INVALID_ARG;
 }
 
@@ -765,7 +883,8 @@ extern "C" int sv_gemm_profile(long long *buf) {
 }
 
 extern "C" int sv_gemm_force_ctas(int ctas) {
-  g_force_bn = ctas & 0xFF;
+  g_force_bn = ctas & 7;
+  g_force_sched = (ctas >> 3) & 3;
   g_gemm_dbg = ctas >> 8;
   return SV_OK;
 }

@@ -118,6 +118,13 @@ __device__ __forceinline__ uint32_t tile_off_sw128(uint32_t rows, uint32_t r, ui
 // named barrier over one warpgroup (ids 1.. ; 0 is __syncthreads)
 __device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
+// move this warpgroup's per-thread register allocation down / up to N (a multiple of 8 in [24, 256]); executed by every thread
+// of the warpgroup.  inc waits until other warpgroups of the CTA have released enough registers.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -234,6 +234,6 @@ def attention_visit_all_blocks(on):
 
 
 def gemm_force_ctas(n):
-    """0 = heuristic, 1 / 2 / 4 = tiles of 64 / 128 / 192 output columns; bits 8.. are timing-only profiling switches
-    (svgps.h)."""
+    """0 = heuristic, 1 / 2 / 4 = tiles of 64 / 128 / 192 output columns, + 8 / + 16 = cooperative / epilogue-warpgroup
+    schedule for staged forwards and dgrads; bits 8.. are timing-only profiling switches (svgps.h)."""
     _lib.check(_lib.gps(), _lib.gps().sv_gemm_force_ctas(int(n)), "sv_gemm_force_ctas")
