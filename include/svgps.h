@@ -231,6 +231,26 @@ int sv_cross_entropy_fwd_bwd_strided(const void *logits, long long row_stride, i
                                      int V, long long ignore_index, float *loss_rows, void *grad_logits,
                                      long long grad_row_stride, void *stream);
 
+/* Masked, mean-normalised softmax cross-entropy, forward + gradient in one launch (reference: optim/loss/loss.py:26-47,
+ * 64-94 — obj_cls_{raw,pre,post}_loss and obj_cls_{pre,post}_loss_{mask,unmask}: F.cross_entropy(logits.permute(0, 2, 1),
+ * obj_labels, reduction='none') * w, summed, divided by w.sum()).  The row body is the one of
+ * sv_cross_entropy_fwd_bwd_strided.  logits (R, row_stride >= V) bf16 (is_bf16 = 1) or f32; labels (R) int64; obj_mask and
+ * sem_mask (R) bytes (bool: nonzero = true).  mode 0: w_r = obj_mask[r]; 1: obj_mask[r] & !sem_mask[r]; 2: obj_mask[r] &
+ * sem_mask[r] (sem_mask may be NULL in mode 0 only).
+ * loss_rows[r] = w_r (logsumexp(row) - row[label]), 0 when the label lies outside [0, V) (torch's ignore_index = -100 of a
+ * padded slot, or any other out-of-range label);  sums[0] = sum_r loss_rows[r], sums[1] = sum_r w_r, *loss_out = sums[0] /
+ * sums[1], written by the last CTA, the rows added in a fixed order (bitwise reproducible, independent of CTA order).
+ * sum_r w_r = 0 (e.g. the _mask loss of a batch with no semantically masked object) gives 0 / 0 = NaN, as in the reference.
+ * A row of weight 0 contributes exactly 0 and its logits are not read; the reference computes CE * 0, which is NaN when
+ * that row's CE is not finite (padded slots have finite logits and label -100, so no input of the pipeline differs).
+ * counter: a zero-initialised device word, left at zero on completion (one per stream).
+ * grad_logits (may be NULL): w_r (softmax(row) - onehot(label)), same dtype, rows grad_row_stride (>= V) elements apart,
+ * columns [V, grad_row_stride) written as zeros — NOT yet divided by sums[1] (sv_scale_inplace does that in the backward). */
+int sv_masked_cross_entropy_fwd_bwd(const void *logits, long long row_stride, int is_bf16, const long long *labels,
+                                    const unsigned char *obj_mask, const unsigned char *sem_mask, int mode, int R, int V,
+                                    float *loss_rows, float *sums, float *loss_out, unsigned *counter, void *grad_logits,
+                                    long long grad_row_stride, void *stream);
+
 /* Binary cross-entropy with logits, forward + gradient in one launch (reference: optim/loss/loss.py:50-53 `answer_loss`, and
  * the ScanQA form of optim/loss/contra_loss.py:33-34 — F.binary_cross_entropy_with_logits(x, y.float(), weight=w,
  * reduction='sum') / R).  logits (R, row_stride >= C) bf16 (is_bf16 = 1) or f32, columns [0, C) used; labels (R, C) int64

@@ -210,6 +210,15 @@ PER_SCENE_UNSUPPORTED = {
     "TextSceneBetweenBatch": "the per-scene model sets no scene_embed / scene_text_embed",
     "answer_loss": "the QA head is given the un-flattened (B, U, T) txt_masks",
     "qa_head": "the QA head is given the un-flattened (B, U, T) txt_masks",
+    "og3d_multi_loss": "BCE over the (B, U, O) per-scene logits needs a target of that shape; the per-scene tgt_object_id "
+                       "is (B, U)",
+    "txt_cls_multi_loss": "no ground head runs per scene, so there are no txt_cls_logits",
+    "obj_cls_pre_loss": "no ground head runs per scene, so there are no obj_cls_pre_logits",
+    "obj_cls_pre_loss_mask": "no ground head runs per scene, so there are no obj_cls_pre_logits",
+    "obj_cls_pre_loss_unmask": "no ground head runs per scene, so there are no obj_cls_pre_logits",
+    "obj_cls_post_loss": "the per-scene obj_cls_post_logits has B*U rows of objects against the (B, O) obj_labels",
+    "obj_cls_post_loss_mask": "the per-scene obj_cls_post_logits has B*U rows of objects against the (B, O) obj_labels",
+    "obj_cls_post_loss_unmask": "the per-scene obj_cls_post_logits has B*U rows of objects against the (B, O) obj_labels",
 }
 
 

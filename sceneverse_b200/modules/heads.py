@@ -3,8 +3,20 @@ import torch
 from torch import nn
 
 from .. import ops
-from .layers import LayerNorm, get_mlp_head
+from .layers import LayerNorm, Linear, get_mlp_head
 from .registry import HEADS_REGISTRY
+
+
+def _class_head(head, x):
+    """A get_mlp_head classifier whose last linear, once routed to the native GEMM (layers.route_linears), runs as
+    ops.padded_vocab_linear: the same values, and a 607-wide output carries its padded parent (`_sv_padded`), which the
+    object-classification losses read in place and return their gradient in."""
+    *body, last = head
+    for m in body:
+        x = m(x)
+    if type(last) is Linear:
+        return ops.padded_vocab_linear(x, last.weight, last.bias)
+    return last(x)
 
 
 @HEADS_REGISTRY.register()
@@ -22,8 +34,8 @@ class GroundHeadV1(nn.Module):
         og3d_logits = og3d_logits.masked_fill_(obj_masks.logical_not(), -float('inf'))
         if self.detach_all_aux_loss:
             txt_embeds, obj_embeds, obj_pre_embeds = txt_embeds.detach(), obj_embeds.detach(), obj_pre_embeds.detach()
-        return (self.txt_clf_head(txt_embeds[:, 0]), self.obj3d_clf_head(obj_embeds),
-                self.obj3d_clf_pre_head(obj_pre_embeds), og3d_logits)
+        return (_class_head(self.txt_clf_head, txt_embeds[:, 0]), _class_head(self.obj3d_clf_head, obj_embeds),
+                _class_head(self.obj3d_clf_pre_head, obj_pre_embeds), og3d_logits)
 
 
 @HEADS_REGISTRY.register()

@@ -1,4 +1,4 @@
-"""Losses on the GPS path (reference: optim/loss/loss.py:8-9,56-61,111-148; optim/loss/contra_loss.py:11-98;
+"""Losses on the GPS path (reference: optim/loss/loss.py:8-94,111-148; optim/loss/contra_loss.py:11-98;
 common/dist_utils.py:131-149)."""
 import numpy as np
 import torch
@@ -45,6 +45,62 @@ def answer_loss(data_dict):
     """loss.py:50-53: BCE with logits over the answer vocabulary against the multi-hot `answer_label` (int64, read as
     float), summed and divided by the batch size; all-zero rows (unanswerable questions) still count."""
     return ops.bce_with_logits_sum(data_dict["answer_scores"], data_dict["answer_label"])
+
+
+def og3d_multi_loss(data_dict):
+    """loss.py:12-16: BCE with logits over `og3d_logits` (B, O) against a multi-hot (B, O) `tgt_object_id` read as float,
+    summed and divided by B.  GroundHeadV1's og3d_logits are -inf at padded objects (heads.py): torch then gives a NaN loss
+    and a zero gradient at those entries, and so does the native kernel; without a ground head the logits are the finite
+    einsum of OpenVocab."""
+    return ops.bce_with_logits_sum(data_dict["og3d_logits"], data_dict["tgt_object_id"])
+
+
+def txt_cls_multi_loss(data_dict):
+    """loss.py:19-23: BCE with logits over `txt_cls_logits` (B, 607) against a multi-hot (B, 607) `tgt_object_label` read as
+    float, summed and divided by B."""
+    return ops.bce_with_logits_sum(data_dict["txt_cls_logits"], data_dict["tgt_object_label"])
+
+
+def obj_cls_raw_loss(data_dict):
+    """loss.py:26-31: (CE(obj_cls_raw_logits) * obj_masks).sum() / obj_masks.sum().  The logits are the detached softmax
+    probabilities of the object encoder's class head (vision.py), so nothing trains on this loss."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_raw_logits"], data_dict["obj_labels"], data_dict["obj_masks"])
+
+
+def obj_cls_pre_loss(data_dict):
+    """loss.py:34-39: (CE(obj_cls_pre_logits) * obj_masks).sum() / obj_masks.sum()."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_pre_logits"], data_dict["obj_labels"], data_dict["obj_masks"])
+
+
+def obj_cls_post_loss(data_dict):
+    """loss.py:42-47: (CE(obj_cls_post_logits) * obj_masks).sum() / obj_masks.sum()."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_post_logits"], data_dict["obj_labels"], data_dict["obj_masks"])
+
+
+def obj_cls_pre_loss_mask(data_dict):
+    """loss.py:64-70: (CE(obj_cls_pre_logits) * w).sum() / w.sum(), w = obj_masks & ~obj_sem_masks (NaN when no object of
+    the batch is semantically masked)."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_pre_logits"], data_dict["obj_labels"], data_dict["obj_masks"],
+                                    data_dict["obj_sem_masks"], mode=1)
+
+
+def obj_cls_pre_loss_unmask(data_dict):
+    """loss.py:72-78: (CE(obj_cls_pre_logits) * w).sum() / w.sum(), w = obj_masks & obj_sem_masks."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_pre_logits"], data_dict["obj_labels"], data_dict["obj_masks"],
+                                    data_dict["obj_sem_masks"], mode=2)
+
+
+def obj_cls_post_loss_mask(data_dict):
+    """loss.py:80-86: (CE(obj_cls_post_logits) * w).sum() / w.sum(), w = obj_masks & ~obj_sem_masks (NaN when no object of
+    the batch is semantically masked)."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_post_logits"], data_dict["obj_labels"], data_dict["obj_masks"],
+                                    data_dict["obj_sem_masks"], mode=1)
+
+
+def obj_cls_post_loss_unmask(data_dict):
+    """loss.py:88-94: (CE(obj_cls_post_logits) * w).sum() / w.sum(), w = obj_masks & obj_sem_masks."""
+    return ops.masked_cross_entropy(data_dict["obj_cls_post_logits"], data_dict["obj_labels"], data_dict["obj_masks"],
+                                    data_dict["obj_sem_masks"], mode=2)
 
 
 def obj_cls_loss(data_dict, smoothing=0.3):

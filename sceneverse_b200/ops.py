@@ -664,6 +664,82 @@ def bce_with_logits_sum(logits, labels, weight=None):
     return F.binary_cross_entropy_with_logits(logits, labels.float(), weight=weight, reduction='sum') / logits.shape[0]
 
 
+_MASKED_CE_COUNTERS = {}
+
+
+class _MaskedCrossEntropyFn(torch.autograd.Function):
+    """sum_r w_r CE_r / sum_r w_r over (R, W) logits; loss, weight sum and unscaled gradient from ONE native launch
+    (sv_masked_cross_entropy_fwd_bwd).  n_classes < W: the trailing columns are padding, ignored by the loss and zero in the
+    gradient.  The backward divides the saved gradient in place by the device weight sum, as _CrossEntropyFn does."""
+
+    @staticmethod
+    def forward(ctx, logits2d, labels, obj_u8, sem_u8, mode, n_classes):
+        from . import _lib
+        R, W = logits2d.shape
+        dev = logits2d.device
+        counter = _MASKED_CE_COUNTERS.get(dev)
+        if counter is None:       # zero-initialised; the kernel leaves it at zero
+            counter = _MASKED_CE_COUNTERS[dev] = torch.zeros(1, dtype=torch.int32, device=dev)
+        loss_rows = torch.empty(R, dtype=torch.float32, device=dev)
+        sums = torch.empty(2, dtype=torch.float32, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        grad = torch.empty((R, W), dtype=logits2d.dtype, device=dev) if logits2d.requires_grad else None
+        _lib.call(_lib.gps(), "sv_masked_cross_entropy_fwd_bwd", dev, logits2d.data_ptr(), logits2d.stride(0),
+                  1 if logits2d.dtype == torch.bfloat16 else 0, labels.data_ptr(), obj_u8.data_ptr(), _lib.ptr(sem_u8),
+                  int(mode), R, n_classes, loss_rows.data_ptr(), sums.data_ptr(), loss.data_ptr(), counter.data_ptr(),
+                  _lib.ptr(grad), W)
+        ctx.save_for_backward(grad, sums[1])
+        ctx.scaled = False
+        return loss
+
+    @staticmethod
+    def backward(ctx, gout):
+        grad, wsum = ctx.saved_tensors
+        return _scale_saved_grad(ctx, "masked_cross_entropy", grad, gout, wsum), None, None, None, None, None
+
+
+def _masked_cross_entropy_torch(logits, labels, obj_masks, sem_masks, mode):
+    """The reference's expression (optim/loss/loss.py:26-47, 64-94), unchanged."""
+    ce = F.cross_entropy(logits.permute(0, 2, 1), labels, reduction='none')
+    if mode == 0:
+        return (ce * obj_masks).sum() / obj_masks.sum()
+    sem = sem_masks.logical_not() if mode == 1 else sem_masks
+    return (ce * obj_masks * sem).sum() / (obj_masks * sem).sum()
+
+
+def masked_cross_entropy(logits, labels, obj_masks, sem_masks=None, mode=0):
+    """The object-classification losses of optim/loss/loss.py: (F.cross_entropy(logits.permute(0, 2, 1), labels,
+    reduction='none') * w).sum() / w.sum() for (B, O, V) logits, (B, O) int64 labels (-100 = padded slot) and (B, O) bool
+    masks, with w = obj_masks (mode 0), obj_masks & ~sem_masks (mode 1, the `_mask` losses) or obj_masks & sem_masks (mode 2,
+    the `_unmask` losses).  w.sum() = 0 gives NaN, as in the reference.  CUDA bf16 / f32 logits: one native launch
+    (sv_masked_cross_entropy_fwd_bwd), reading a padded-vocabulary row (`_sv_padded`) in place and returning the gradient in
+    that layout, no gradient buffer when the logits need none; anything else: the reference's torch expression."""
+    if mode not in (0, 1, 2):
+        raise ValueError(f"masked_cross_entropy: mode must be 0, 1 or 2, got {mode!r}")
+    if mode != 0 and sem_masks is None:
+        raise ValueError("masked_cross_entropy: modes 1 and 2 need sem_masks")
+    if logits.dim() != 3 or labels.shape != logits.shape[:2] or obj_masks.shape != labels.shape or \
+            (sem_masks is not None and sem_masks.shape != labels.shape):
+        raise ValueError(f"masked_cross_entropy: logits {tuple(logits.shape)} must be (B, O, V) with labels "
+                         f"{tuple(labels.shape)}, obj_masks {tuple(obj_masks.shape)} and sem_masks "
+                         f"{None if sem_masks is None else tuple(sem_masks.shape)} all (B, O)")
+    B, O, V = logits.shape
+    src = logits
+    padded = getattr(logits, "_sv_padded", None)
+    if padded is not None and padded.dim() == 3 and padded.shape[:2] == (B, O) and padded.is_contiguous():
+        src = padded
+    src2d = src.reshape(B * O, src.shape[-1]) if src.stride(-1) == 1 else None
+    native = src2d is not None and src2d.is_cuda and src2d.dtype in (torch.bfloat16, torch.float32) and \
+        src2d.stride(1) == 1 and B * O > 0 and labels.is_cuda and labels.dtype == torch.int64 and \
+        obj_masks.is_cuda and obj_masks.dtype in (torch.bool, torch.uint8) and \
+        (mode == 0 or (sem_masks.is_cuda and sem_masks.dtype in (torch.bool, torch.uint8)))
+    if not native:
+        return _masked_cross_entropy_torch(logits, labels, obj_masks, sem_masks, mode)
+    obj_u8 = obj_masks.contiguous().view(torch.uint8).reshape(-1)
+    sem_u8 = None if mode == 0 else sem_masks.contiguous().view(torch.uint8).reshape(-1)
+    return _MaskedCrossEntropyFn.apply(src2d, labels.reshape(-1).contiguous(), obj_u8, sem_u8, mode, V)
+
+
 class _AttentionPoolFn(torch.autograd.Function):
     """pooled = sum_l softmax_l(masked score) x_l for one glimpse (modules/heads/qa_head.py:57-69), one native launch per
     direction.  `scores` is the PADDED (B, L, 8) output of the N = 1 score linear; its gradient is returned in that layout."""

@@ -81,13 +81,18 @@ def adversarial_clouds(seed, N):
     return out
 
 
-def scene_batch(seed, B=64, O=80, P=1024, L=50, Ls=300, min_obj=8, all_valid=False, max_obj=None):
+def scene_batch(seed, B=64, O=80, P=1024, L=50, Ls=300, min_obj=8, all_valid=False, max_obj=None, multi_target=False,
+                multi_label=False):
     """Synthetic `data_dict` with the key set / dtypes of the reference's dataset wrappers
     (data/datasets/dataset_wrapper.py:38-111,147-195; SURVEY.md §8a row D), as numpy arrays:
     txt_ids/txt_masks (B,L) int64, obj_fts (B,O,P,6) f32 (padded objects all 1.0), obj_locs (B,O,6) f32 (pad 0),
     obj_masks/obj_sem_masks (B,O) bool, obj_labels (B,O) int64 (pad -100), tgt_object_id (B,1) int64,
     masked_lm_labels (B,L) int64 (-1 = ignore), scene_txt_ids/scene_txt_masks (B,Ls) int64.
-    Each scene has between min_obj and max_obj (default O) valid objects."""
+    Each scene has between min_obj and max_obj (default O) valid objects.
+    The multi-hot targets of the reference's multi-target losses (optim/loss/loss.py:12-23), drawn from a separate RNG
+    stream, so the other arrays of a seed are unchanged:
+    multi_target=True: tgt_object_id is (B, O) int64 multi-hot over 1-3 valid objects, the (B, 1) target among them;
+    multi_label=True: tgt_object_label (B, 607) int64 multi-hot at the targets' obj_labels."""
     rng = np.random.default_rng(seed)
     d = {}
     hi = O if max_obj is None else max_obj
@@ -126,6 +131,21 @@ def scene_batch(seed, B=64, O=80, P=1024, L=50, Ls=300, min_obj=8, all_valid=Fal
     lm[pick] = d["txt_ids"][pick]
     d["masked_lm_labels"] = lm
     d["scene_txt_ids"], d["scene_txt_masks"] = text(Ls)
+    if multi_target or multi_label:
+        mrng = np.random.default_rng([seed, 0xA11])
+        tgt = np.zeros((B, O), np.int64)
+        tgt[np.arange(B), d["tgt_object_id"][:, 0]] = 1
+        if multi_target:
+            for b in range(B):
+                n = int(n_obj[b])
+                tgt[b, mrng.choice(n, size=int(mrng.integers(0, min(2, n - 1) + 1)), replace=False)] = 1
+        if multi_label:
+            lab = np.zeros((B, 607), np.int64)
+            for b in range(B):
+                lab[b, obj_labels[b][tgt[b] == 1]] = 1
+            d["tgt_object_label"] = lab
+        if multi_target:
+            d["tgt_object_id"] = tgt
     return d
 
 
